@@ -66,8 +66,10 @@ struct SolveSmem {
     int *rp, *fst;   // row pointers (nf + 1) and first columns (nf)
     double *g, *sc, *D, *sg, *y, *u, *Hu, *ug, *uvis, *red, *bc, *chol, *dinv, *xo, *Pt;
     int *amap, *vmap;
+    unsigned char *tl;   // per Cholesky panel: the count, then the trailing 4-row groups that reach the panel (chol_tile_lists)
 };
-VIWB_HD size_t solve_smem_doubles(int nt, int esize) { return (size_t)((esize + 1) & ~1) + 9 * TFIX + 2 * VSUB + 5 * 32 + 16 + 2 * TFIX + 2 + (size_t)((nt + 31) / 32) * 48 + 2 * TFIX + 8 * (TFIX + 4) + 2; }   // ints: amap, vmap, rp, fst
+enum { CHOL_TLD = 52 };  // bytes per panel in tl: the count + up to (TFIX + 4) / 4 = 49 groups
+VIWB_HD size_t solve_smem_doubles(int nt, int esize) { return (size_t)((esize + 1) & ~1) + 9 * TFIX + 2 * VSUB + 5 * 32 + 16 + 2 * TFIX + 2 + (size_t)((nt + 31) / 32) * 48 + 2 * TFIX + 8 * (TFIX + 4) + 2 + TFIX / 8 * CHOL_TLD / 8; }   // ints: amap, vmap, rp, fst; bytes: tl
 VIWB_D void carve(SolveSmem &s, double *smem, int nt, int esize) {
     double *p = smem;
     s.L = p; p += (size_t)((esize + 1) & ~1);
@@ -80,6 +82,7 @@ VIWB_D void carve(SolveSmem &s, double *smem, int nt, int esize) {
     if ((p - smem) & 1) p++;                    // Pt is read with 16-byte vector loads
     s.Pt = p; p += 8 * (TFIX + 4);
     s.amap = (int *)p; s.vmap = s.amap + TFIX; s.rp = s.vmap + TFIX; s.fst = s.rp + TFIX + 2;
+    s.tl = (unsigned char *)(p + 2 * TFIX + 2);
 }
 // entry (i, j), j <= i, of the skyline; must lie inside the envelope
 #define SKY(s, i, j) ((s).L[(s).rp[i] - (s).fst[i] + (j)])
@@ -165,7 +168,25 @@ VIWB_D void load4(const double *p, double *o) {
     o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
 #endif
 }
-VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double *y, int n, int tid, int nt, double *scratch, double *dinv, double *Pt) {
+// Per panel (trailing rows r0.. = c0 + nb..), the 4-row groups ti (rows r0 + 4 ti ..) holding a row that reaches the panel (first stored
+// column < r0; row n, the right-hand side, always does): the trailing update enumerates only the tiles between two such groups.  The
+// lists depend on the skyline alone and are built once per launch.
+template <typename Fst>
+VIWB_D void chol_tile_lists(const Fst *fst, int n, unsigned char *tl, int tid, int nt) {
+    for (int p = tid; p * CHOL_NB < n; p += nt) {
+        const int c0 = p * CHOL_NB, r0 = c0 + ((n - c0) < CHOL_NB ? (n - c0) : CHOL_NB), mt = (n + 1 - r0 + 3) / 4;
+        unsigned char *lp = tl + p * CHOL_TLD;
+        int na = 0;
+        for (int ti = 0; ti < mt; ti++) {
+            bool hit = false;
+            for (int a = 0; a < 4; a++) { const int i = r0 + 4 * ti + a; if (i <= n && (i == n || fst[i] < r0)) hit = true; }
+            if (hit) lp[1 + na++] = (unsigned char)ti;
+        }
+        lp[0] = (unsigned char)na;
+    }
+}
+VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double *y, int n, int tid, int nt, double *scratch, double *dinv, double *Pt,
+                                const unsigned char *tl) {
     // skyline rows: ROW(i)[j] is entry (i, j) for fst[i] <= j <= i; row n is the right-hand side (dense).  FST(i) = first stored column.
 #define ROW(i) ((i) < n ? L + rp[i] - fst[i] : y)
 #define FST(i) ((i) < n ? fst[i] : 0)
@@ -251,15 +272,18 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
         // factored diagonal block back into the matrix (only now: the other warps have finished reading the unfactored one)
         for (int r = tid; r < nb; r += nt) { double *rk = ROW(c0 + r) + c0; const int fr = FST(c0 + r); for (int j = 0; j <= r; j++) if (c0 + j >= fr) rk[j] = my[r * (r + 1) / 2 + j]; }
         // trailing update with 4x4 register tiles over rows i in [r0, n], columns k in [r0, min(i, n-1)]; a tile whose row group or
-        // column group lies entirely right of the panel (first stored column >= r0) has nothing to receive
-        const int ntile = mt * (mt + 1) / 2;
+        // column group lies entirely right of the panel (first stored column >= r0) has nothing to receive: only the row groups of the
+        // panel's list are paired, and a column group that reaches the panel through row n alone is skipped
+        const unsigned char *lp = tl + (c0 / CHOL_NB) * CHOL_TLD;
+        const int na = lp[0], ntile = na * (na + 1) / 2;
         for (int t = tid; t < ntile; t += nt) {
-            int ti, tk; sym_unrank(t, ti, tk);
+            int ai, ak; sym_unrank(t, ai, ak);
+            const int ti = lp[1 + ai], tk = lp[1 + ak];
             const int ib = r0 + 4 * ti, kb = r0 + 4 * tk;
-            bool hit_i = false, hit_k = false;
+            bool hit_k = false;
 #pragma unroll
-            for (int a = 0; a < 4; a++) { if (ib + a <= n && FST(ib + a) < r0) hit_i = true; if (kb + a < n && FST(kb + a) < r0) hit_k = true; }
-            if (!hit_i || !hit_k) continue;
+            for (int a = 0; a < 4; a++) if (kb + a < n && FST(kb + a) < r0) hit_k = true;
+            if (!hit_k) continue;
             double acc[16];
 #pragma unroll
             for (int q = 0; q < 16; q++) acc[q] = 0.0;
@@ -341,6 +365,24 @@ VIWB_D void chol_backsolve_blocked(const double *L, const int *rp, const int *fs
 
 VIWB_D void terminate(WinWork &ww, int term) { ww.status = ST_DONE; ww.term = term; }
 
+enum { SCHUR_U = 4 };      // envelope entries per thread and trip of the Schur subtraction
+
+// Phase probe (measurement build only, `make phases` -> libviwb_phases.so): thread 0 reads clock64() at the barrier-delimited phase
+// boundaries of a launch that computes a step and adds the cycles since the previous boundary to its window's slot of the phase.
+// Launches that only decide the pending candidate and stop are not counted.  The product library compiles none of this.
+enum { SPH_PRO, SPH_ASM, SPH_DSC, SPH_CAUCHY, SPH_SCHUR, SPH_CHOL, SPH_BACK, SPH_LM2, SPH_FORMS, SPH_DOGLEG, SPH_N,
+       SPH_STEPS = SPH_N, SPH_FACT, SPH_SLOTS, SPH_MAXW = 8192 };
+#if defined(VIWB_SOLVE_PROBE) && !defined(VIWB_HOST_EMU)
+__device__ unsigned long long g_solve_phase[SPH_MAXW * SPH_SLOTS];
+#define SOLVE_PROBE_START() long long sph_t = clock64()
+#define SOLVE_MARK(p) do { if (tid == 0 && w < SPH_MAXW) { const long long t_ = clock64(); g_solve_phase[w * SPH_SLOTS + (p)] += t_ - sph_t; sph_t = t_; } } while (0)
+#define SOLVE_COUNT(p) do { if (tid == 0 && w < SPH_MAXW) g_solve_phase[w * SPH_SLOTS + (p)]++; } while (0)
+#else
+#define SOLVE_PROBE_START() ((void)0)
+#define SOLVE_MARK(p) ((void)0)
+#define SOLVE_COUNT(p) ((void)0)
+#endif
+
 // max |x - Plus(x, -g)| over one fixed block (ambient infinity norm of the projected gradient step)
 VIWB_D double block_grad_inf(int b, unsigned mask, const double *x, const double *gneg) {
     const int gs = blk_size(b);
@@ -371,12 +413,14 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
     double *Hpk = bd.Hpk + (size_t)w * (TFIX * (TFIX + 1) / 2), *gpk = bd.gpk + (size_t)w * TFIX;
     const double *Tvis = bd.Tvis + (size_t)w * VSUB * VSUB, *tvec = bd.tvec + (size_t)w * VSUB;
     const double min_mu = 1e-8, max_mu = 1.0, mu_inc = 10.0;
+    SOLVE_PROBE_START();
 
     // compact <-> fixed / visual index maps
     for (int b = tid; b < NB; b += nt) if (m.tcol[b] >= 0) for (int k = 0; k < blk_tsize(b); k++) {
         s.amap[m.tcol[b] + k] = blk_toff(b) + k;
         s.vmap[m.tcol[b] + k] = blk_voff(b) >= 0 ? blk_voff(b) + k : -1;
     }
+    chol_tile_lists(m.efirst, nf, s.tl, tid, nt);
     VIWB_SYNC();
 
     if (mode == 2) { assemble_H(bd, w, s, nf, Hpk, gpk, tid, nt); return; }     // debug hook: normal equations only
@@ -435,12 +479,14 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
     for (;;) {
         if (tid == 0) ww.iteration++;
         VIWB_SYNC();
+        SOLVE_MARK(SPH_PRO);
         bool ls_failure = false;
         if (!ww.reuse) {
             VIWB_SYNC();
             if (tid == 0) ww.reuse = 1;
             if (!assembled) { assemble_H(bd, w, s, nf, Hpk, gpk, tid, nt); assembled = true; }
             else { load_H(Hpk, s, nf, tid, nt); for (int i = tid; i < nf; i += nt) s.g[i] = gpk[i]; VIWB_SYNC(); }
+            SOLVE_MARK(SPH_ASM);
             if (ww.first) {
                 for (int i = tid; i < nf; i += nt) g_scale[i] = op.jacobi_scaling ? 1.0 / (1.0 + sqrt(SKY(s, i, i))) : 1.0;
             }
@@ -476,6 +522,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 const double sg = c * lm_g[k] / D; g_sg[TFIX + k] = sg; n2 += sg * sg;
             }
             n2 = block_sum(n2, tid, nt, s.red);
+            SOLVE_MARK(SPH_DSC);
             // q_gg = |J u_g|^2, l_g = g . u_g
             symv(s, nf, s.ug, s.Hu, tid, nt);
             to_vis(s, nf, s.ug, s.uvis, tid, nt);
@@ -495,6 +542,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
             { double v2[2] = {q, l}; block_sum_n<2>(v2, tid, nt, s.red); q = v2[0]; l = v2[1]; }
             if (tid == 0) { ww.sgrad_norm = sqrt(n2); ww.q_gg = q; ww.l_g = l; ww.alpha = n2 / q; }
             VIWB_SYNC();
+            SOLVE_MARK(SPH_CAUCHY);
             // ---- Gauss-Newton step: (J^T J + mu D^2) y = J^T r through the Schur complement
             ls_failure = true;
             bool h_dirty = false;
@@ -502,17 +550,39 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 if (h_dirty) load_H(Hpk, s, nf, tid, nt);
                 const double mu = ww.mu;
                 const bool t_ok = (mu == ww.mu_lin);          // gamma / T / tvec were built for mu_lin
-                // S = C (H - T) C + mu D^2 ; rhs = C (g - tvec)     (one warp per skyline row, lanes over its stored columns)
+                // S = C (H - T) C + mu D^2 ; rhs = C (g - tvec)     (entry-parallel over the envelope: a thread takes SCHUR_U entries
+                // per trip, finds their rows by bisection of rp and issues all their T loads before it updates the first one)
                 {
-                    const int Wd = nt < 32 ? nt : 32, nwp = nt / Wd, wid = tid / Wd, ln = tid % Wd;
-                    for (int i = wid; i < nf; i += nwp) {
+                    for (int i = tid; i < nf; i += nt) {
                         const int vi = s.vmap[i];
-                        double *ri = s.L + s.rp[i] - s.fst[i];
-                        for (int j = s.fst[i] + ln; j <= i; j += Wd) {
-                            const int vj = s.vmap[j];
-                            double hij = ri[j];
+                        double r = s.g[i];
+                        if (vi >= 0) {
+                            if (t_ok) r -= tvec[vi];
+                            else { double t = 0.0; for (int k = 0; k < N; k++) { const double c = lm_sc[k], sk = c * c * lm_a[k], Dk = g_D[TFIX + k]; t += (c * c / (sk + mu * Dk * Dk)) * W[(size_t)k * VSUB + vi] * lm_g[k]; } r -= t; }
+                        }
+                        s.y[i] = s.sc[i] * r;
+                    }
+                    const int ne = s.rp[nf];
+                    for (int e0 = tid; e0 < ne; e0 += SCHUR_U * nt) {
+                        int ii[SCHUR_U], jj[SCHUR_U];
+                        double tv[SCHUR_U];
+#pragma unroll
+                        for (int u = 0; u < SCHUR_U; u++) {
+                            const int e = e0 + u * nt;
+                            int lo = 0, hi = nf;                    // row: the last i with rp[i] <= e
+                            if (e < ne) while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (s.rp[mid] <= e) lo = mid; else hi = mid; }
+                            ii[u] = lo; jj[u] = s.fst[lo] + e - s.rp[lo];
+                            const int vi = s.vmap[lo], vj = e < ne ? s.vmap[jj[u]] : -1;
+                            tv[u] = (t_ok && vi >= 0 && vj >= 0) ? Tvis[vi * VSUB + vj] : 0.0;
+                        }
+#pragma unroll
+                        for (int u = 0; u < SCHUR_U; u++) {
+                            const int e = e0 + u * nt, i = ii[u], j = jj[u];
+                            if (e >= ne) break;
+                            const int vi = s.vmap[i], vj = s.vmap[j];
+                            double hij = s.L[e];
                             if (vi >= 0 && vj >= 0) {
-                                if (t_ok) hij -= Tvis[vi * VSUB + vj];
+                                if (t_ok) hij -= tv[u];
                                 else {
                                     double t = 0.0;
                                     for (int k = 0; k < N; k++) {
@@ -524,25 +594,20 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                             }
                             hij *= s.sc[i] * s.sc[j];
                             if (i == j) hij += mu * s.D[i] * s.D[i];
-                            ri[j] = hij;
+                            s.L[e] = hij;
                         }
-                    }
-                    for (int i = tid; i < nf; i += nt) {
-                        const int vi = s.vmap[i];
-                        double r = s.g[i];
-                        if (vi >= 0) {
-                            if (t_ok) r -= tvec[vi];
-                            else { double t = 0.0; for (int k = 0; k < N; k++) { const double c = lm_sc[k], sk = c * c * lm_a[k], Dk = g_D[TFIX + k]; t += (c * c / (sk + mu * Dk * Dk)) * W[(size_t)k * VSUB + vi] * lm_g[k]; } r -= t; }
-                        }
-                        s.y[i] = s.sc[i] * r;
                     }
                 }
                 VIWB_SYNC();
+                SOLVE_MARK(SPH_SCHUR);
+                SOLVE_COUNT(SPH_FACT);
                 h_dirty = true;
                 if (tid == 0) ww.num_linear++;
-                bool ok = cholesky_packed_rhs(s.L, s.rp, s.fst, s.y, nf, tid, nt, s.chol, s.dinv, s.Pt);
+                bool ok = cholesky_packed_rhs(s.L, s.rp, s.fst, s.y, nf, tid, nt, s.chol, s.dinv, s.Pt, s.tl);
+                SOLVE_MARK(SPH_CHOL);
                 if (ok) {
                     chol_backsolve_blocked(s.L, s.rp, s.fst, s.y, s.dinv, s.xo, nf, tid, nt);
+                    SOLVE_MARK(SPH_BACK);
                     // back-substitute the inverse depths (scaled): y_k = (c g_k - c w_k . (C y_f)) / h_k
                     for (int i = tid; i < nf; i += nt) s.u[i] = s.sc[i] * s.y[i];
                     VIWB_SYNC();
@@ -562,6 +627,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                     }
                     bad = block_sum(bad, tid, nt, s.red);
                     ok = (bad == 0.0);
+                    SOLVE_MARK(SPH_LM2);
                 }
                 if (!ok) { VIWB_SYNC(); if (tid == 0) ww.mu *= mu_inc; VIWB_SYNC(); continue; }
                 ls_failure = false;
@@ -593,6 +659,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 if (tid == 0) { ww.q_nn = qnn; ww.q_gn = qgn; ww.l_n = ln; ww.gn_norm = sqrt(nn); ww.sgrad_dot_gn = gd; }
             }
             VIWB_SYNC();
+            SOLVE_MARK(SPH_FORMS);
             if (tid == 0) ww.first = 0;
             VIWB_SYNC();
         }
@@ -657,6 +724,8 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
             ww.phase = PH_CAND;
             ww.mu_lin = fmax(min_mu, 2.0 * ww.mu / mu_inc);      // the candidate's linearisation is solved with the post-accept mu
         }
+        SOLVE_MARK(SPH_DOGLEG);
+        SOLVE_COUNT(SPH_STEPS);
         return;
     }
 }

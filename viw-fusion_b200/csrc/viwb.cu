@@ -980,6 +980,26 @@ extern "C" int viwb_profile_get(viwb_context *ctx, int idx, char *name, int name
 #endif
 }
 
+#if defined(VIWB_SOLVE_PROBE) && !defined(VIWB_HOST_EMU)
+// phase probe of the solve kernel (libviwb_phases.so only; profiles/solve_phase_probe.py): per window, SPH_SLOTS counters --
+// the cycles of each phase summed over the launches that computed a step, then the number of such launches and of factorisations
+extern "C" int viwb_solve_probe_slots(void) { return SPH_SLOTS; }
+extern "C" int viwb_solve_probe_clear(viwb_context *ctx) {
+    bind_device(ctx);
+    CK(cudaStreamSynchronize(ctx->stream));
+    static const std::vector<unsigned long long> zero((size_t)SPH_MAXW * SPH_SLOTS, 0ull);
+    CK(cudaMemcpyToSymbol(g_solve_phase, zero.data(), zero.size() * sizeof(unsigned long long)));
+    return VIWB_OK;
+}
+extern "C" int viwb_solve_probe_read(viwb_context *ctx, int nwin, unsigned long long *out) {
+    bind_device(ctx);
+    if (nwin < 0 || nwin > SPH_MAXW) return fail(ctx, VIWB_ERR_INVALID, "viwb_solve_probe_read: nwin out of range");
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaMemcpyFromSymbol(out, g_solve_phase, (size_t)nwin * SPH_SLOTS * sizeof(unsigned long long)));
+    return VIWB_OK;
+}
+#endif
+
 extern "C" int viwb_batch_create(viwb_context *ctx, int batch, const viwb_problem *problems, const double *const *states,
                                  const viwb_options *options, const int32_t *margin_flags, viwb_batch **out) {
     if (!ctx || !out) return VIWB_ERR_INVALID;
