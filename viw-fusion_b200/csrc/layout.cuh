@@ -33,11 +33,17 @@ VIWB_HD int blk_msize(int b) { int s = blk_size(b); return s == 7 ? 6 : s; }
 VIWB_HD int blk_voff(int b) { return b < 11 ? 6 * b : b == BLK_EX0 ? 66 : b == BLK_EX1 ? 72 : b == BLK_TD ? 78 : -1; }
 
 enum { ASM_STRIDE = 108, ASM_CHUNK = 256, ITEM_FRAME = 0, ITEM_PAIR = 1, ITEM_COMMON = 2 };
-// Fused path (solver linearisation of batches whose windows keep ex0 / ex1 / td constant): lin_vis_lm evaluates the factors of whole landmarks per
-// block and leaves one X record per two-frame factor, X = [A | B | r] (2 x 13, row stride 14), at the factor's position in FRAME-PAIR order; asm_pairs
-// turns the records of one (host, observer) pair into G = sum X^T X (13 x 13 inside three 8 x 8 FP64 tensor-core tiles) per chunk of PAIR_CHUNK records.
+// Fused path (solver linearisation of windows whose ex0 / ex1 / td are constant, "compact"): lin_vis_lm walks one HOST RUN per block -- the landmarks
+// hosted in one frame, in landmark order, as tiles of whole landmarks -- and forms G = sum X^T X of every (host, observer) pair straight from the
+// shared-memory tile (X = [A | B | r], 2 x 13; G: 13 x 13 inside three 8 x 8 FP64 tensor-core tiles), per chunk of PAIR_CHUNK records of the pair.
+// Wide solver windows and every marginalisation keep landmark blocks (LmbDesc): lin_vis_lm_wide stores X records in frame-pair order, asm_pairs_wide
+// turns them into the same chunk products.
 enum { PAIR_CHUNK = 64, LMB_FACTORS = 128, NPAIR = NFR * (NFR - 1) / 2, PAIR_RED = NFR * 105 + NPAIR * 36 + 104 + 1 };      // PAIR_RED: the WIDE pair_reduce output (the compact one is a prefix-sized subset)
 struct alignas(32) LmbDesc { int win, k0, k1, f0, nf, pad[3]; };      // window, global landmark range [k0, k1), first factor (global) and factor count (<= LMB_FACTORS)
+// host run: window, host frame, its tiles [t0, t0 + ntile) in run_tile, and per observer frame j the pair item (global index into pitems / pair_out)
+// of the first chunk of pair (host, j), -1 if the window has no such record
+struct alignas(16) RunDesc { int win, host, t0, ntile, pfirst[NFR], pad; };
+struct RunTile { int l0, nl, f0, nf; };      // entries [l0, l0 + nl) of run_lm and [f0, f0 + nf) of run_f (nf <= LMB_FACTORS)
 struct AsmItem { int kind, win, a, b, lo, hi, phase, has_common, base; };      // base: fused path, offset (doubles) of the window's record region in xrec
 
 struct PriorDev {       // one per window that has a valid prior
@@ -60,10 +66,10 @@ struct WinMeta {        // read-only during a solve
     int item_off, nitems, nphases, list_off;     // assembly items of the solver linearisation (kernels_asm.cuh); list entries are window-local
     int mitem_off, nmitems, nmphases, mlist_off; // assembly items of the marginalisation linearisation (factors hosted in frame 0)
     int has_common;                     // any of ex0 / ex1 / td is an active column (solver); marginalisation always counts them
-    int xrec_off, nxrec;                // fused path (solver): the window's record region in xrec (offset in DOUBLES), number of records
+    int xrec_off, nxrec;                // fused path (wide solver windows): the window's record region in xrec (offset in DOUBLES), number of records
     int pitem_off, npitems;             // fused path: pair items (chunks of one frame pair's records), head item of a pair has phase 0
-    int lmb_off, nlmb;                  // landmark blocks (whole landmarks, <= LMB_FACTORS factors) of lin_vis_lm, solver and marginalisation
-    int fused;                          // 1: this window's solver linearisation takes the fused path (regular factor table); records COMPACT unless has_common
+    int lmb_off, nlmb;                  // landmark blocks (whole landmarks, <= LMB_FACTORS factors) of lin_vis_lm_wide, solver (wide windows) and marginalisation
+    int fused;                          // 1: this window's solver linearisation takes the fused path (regular factor table): host runs unless has_common
     int mxrec_off, nmxrec, mpitem_off, nmpitems;      // fused marginalisation (MARGIN_OLD, regular table): WIDE records of the factors hosted in frame 0, their pair items
     int mfused;
     short tcol[NB];     // compact column of fixed block b, -1 if constant / absent / unreferenced
@@ -101,15 +107,20 @@ struct BatchDev {       // passed by value to every kernel
     int env_max;            // largest esize over the batch (sizes the solve kernel's shared memory)
     int marg_nmax;          // largest prior dimension any window of the batch produces (sizes the eigen-solver's shared memory)
     int rec_stride_solve;   // VREC_COMPACT if no window of the batch has ex0/ex1/td active, else VREC (marginalisation always uses VREC)
-    int n_unfused;          // windows whose solver linearisation runs lin_vis + lm_reduce + asm_items (the others: lin_vis_lm + asm_pairs, WinMeta.fused)
+    int n_unfused;          // windows whose solver linearisation runs lin_vis + lm_reduce + asm_items (the others: lin_vis_lm(_wide), WinMeta.fused)
     int n_fused_wide, n_fused_compact, n_munfused, n_mfused;      // fused solver windows by record width; marginalising windows by path
     int nlmb_total, npitems_total, nmpitems_total, pitems_max;
-    int pwin_smem, pwin_smem_marg;      // dynamic shared memory of pair_win (solver / marginalisation mode); 0: a window's chunks do not fit, asm_pairs + pair_reduce run instead
+    int pwin_smem, pwin_smem_marg;      // dynamic shared memory of pair_win (solver / marginalisation mode); 0: a window's chunks do not fit (or, solver, compact windows form theirs in lin_vis_lm), asm_pairs_wide + pair_reduce run instead
     int pout_stride;        // doubles per solver pair item in pair_out: 192 (all fused windows compact) or 640
     const int *mvis_pos;            // [nvis_total] marginalisation: window-local record slot of the factors hosted in frame 0 (-1 otherwise)
     const struct AsmItem *mpitems;  // [nmpitems_total]
     double *mpair_out;              // [nmpitems_total][640]
-    const int *vis_pos;             // [nvis_total] window-local position of the factor's X record in frame-pair order, -1 for one-frame factors
+    const int *vis_pos;             // [nvis_total] wide solver windows: window-local position of the factor's X record in frame-pair order (-1: none)
+    int nrun_total;                 // host runs of the compact solver windows, longest first (the blocks of lin_vis_lm)
+    const struct RunDesc *run_desc; // [nrun_total]
+    const struct RunTile *run_tile; // tiles of every run, consecutive per run
+    const int *run_f;               // [nvis_total] compact windows: the window's factors (global index) in run order, at the window's vis_off
+    const int *run_lm;              // [nlm_total][2] compact windows: landmark (global) and its first row in its tile, in run order, at the window's lm_off
     unsigned char *vis_dup;         // [nvis_total] 0: the factor alone observes its landmark from frame j; 1: first of two such factors (adds the next one's part); 2: second (adds nothing)
     const struct LmbDesc *lmb_desc; // [nlmb_total] landmark blocks of lin_vis_lm: everything the block needs to start, in one 32-byte load
     double *xrec;                   // [nxrec_total][XREC]

@@ -115,7 +115,6 @@ DEF_KERNEL2(solve, SOLVE_NT, 2)
 #endif
 DEF_KERNEL2(lin_vis_lm, LMB_FACTORS, LVL_MINB)
 DEF_KERNEL2(lin_vis_lm_wide, LMB_FACTORS, 3)
-DEF_KERNEL(asm_pairs, 128)
 DEF_KERNEL(asm_pairs_wide, 128)
 #ifndef PAIR_RED_NT
 #define PAIR_RED_NT 256
@@ -243,7 +242,9 @@ struct WinLow {
     int nlist_s, nitems_s, nph_s, nlist_m, nitems_m, nph_m;
     int prior_n_out;
     bool regular;               // fused path possible: grouped table, <= LMB_FACTORS factors per landmark, at most two factors per (landmark, observer), consecutive
-    int nlmb, npitems, nxrec;   // landmark blocks of lin_vis_lm, pair chunks of asm_pairs, records (two-frame factors; + the one-frame ones when the records are wide)
+    int nlmb, npitems, nxrec;   // landmark blocks of lin_vis_lm_wide, pair chunks, wide records (two-frame factors + the one-frame ones)
+    int nrun, nrtile, rtile_off;              // compact windows: host runs of lin_vis_lm, their tiles, the first tile's index
+    int run_nt[NFR], run_slot[NFR];           // per host frame: tiles of its run, the run's descriptor index (runs are ordered longest first)
     int nmpitems, nmxrec;       // the same for the marginalisation of frame 0 (factors hosted there, wide records)
     bool obs_per_factor; int nobs_i, obsi_off;       // entries of the host-side observation table (wire format): one per run of factors with an identical (pts_i, velocity_i, td_i)
 };
@@ -254,6 +255,27 @@ static inline bool same_host_side(const double *a, const double *b) {      // bi
     return ((bits(a) ^ bits(b)) | (bits(a + 1) ^ bits(b + 1)) | (bits(a + 2) ^ bits(b + 2)) | (bits(a + 6) ^ bits(b + 6)) | (bits(a + 7) ^ bits(b + 7)) | (bits(a + 10) ^ bits(b + 10))) == 0;
 }
 static void split_obs(const double *o, double *hi, double *hj) { hi[0] = o[0]; hi[1] = o[1]; hi[2] = o[2]; hi[3] = o[6]; hi[4] = o[7]; hi[5] = o[10]; hj[0] = o[3]; hj[1] = o[4]; hj[2] = o[5]; hj[3] = o[8]; hj[4] = o[9]; hj[5] = o[11]; }
+
+// Host runs of a compact fused window (kernels_fused.cuh, lin_vis_lm): per host frame, ascending, the landmarks it hosts in landmark order, cut into
+// tiles of whole landmarks with at most LMB_FACTORS factors.  A landmark without factors joins the run of the lowest host frame, so that its outputs
+// are still written.  A host's landmarks need not be consecutive: each run is a list.  visit(host, landmark, first factor, factor count, opens a tile)
+// is called for every landmark, run by run, in run order.  vl / vi: the grouped factor table's landmarks and host frames.
+template <typename F> static void host_runs(int nvis, const int *vl, const int *vi, int nlm, F visit) {
+    static thread_local std::vector<int> first, cnt;
+    first.assign(nlm > 0 ? nlm : 1, 0); cnt.assign(nlm > 0 ? nlm : 1, 0);
+    int h0 = NFR;
+    for (int i = 0; i < nvis; i++) { if (cnt[vl[i]]++ == 0) first[vl[i]] = i; h0 = std::min(h0, vi[i]); }
+    for (int h = h0; h < NFR; h++) {
+        int in_tile = 0; bool open = false;
+        for (int k = 0; k < nlm; k++) {
+            if ((cnt[k] ? vi[first[k]] : h0) != h) continue;
+            const bool fresh = !open || in_tile + cnt[k] > LMB_FACTORS;
+            if (fresh) { in_tile = 0; open = true; }
+            in_tile += cnt[k];
+            visit(h, k, first[k], cnt[k], fresh);
+        }
+    }
+}
 
 static void lower_count(const viwb_problem &p, int mf, WinMeta &m, WinLow &lo, int &out_mode) {
     memset(&m, 0, sizeof m); memset(&lo, 0, sizeof lo);
@@ -412,6 +434,10 @@ static void lower_count(const viwb_problem &p, int mf, WinMeta &m, WinLow &lo, i
             in_blk += cnt;
         }
     }
+    if (lo.regular && !m.has_common) {      // compact records: the pairs' products are formed per host run, no record is stored
+        lo.nxrec = 0;
+        host_runs(p.num_vis, p.vis_landmark, p.vis_frame_i, p.num_landmarks, [&](int h, int, int, int, bool fresh) { if (fresh) { if (lo.run_nt[h]++ == 0) lo.nrun++; lo.nrtile++; } });
+    }
 }
 
 // ---- phase 3: fill this window's slices of the (pinned) staging arrays; every offset is final
@@ -421,6 +447,7 @@ struct HostArrays {
     double *imu_data, *wheel_data, *prior_J, *prior_r, *prior_x0, *x_init; WinWork *work;
     int nitems_solve_total;
     int *vis_pos; LmbDesc *lmb_desc; AsmItem *pitems; int *mvis_pos; AsmItem *mpitems;
+    RunDesc *run_desc; RunTile *run_tile; int *run_f, *run_lm;
     unsigned char *obs_viol;        // [B] host only: set by lower_fill when a grouped table does not share one host-side observation per landmark
 };
 static void emit_lists(const int *type, const int *fi, const int *fj, int nvis, bool only_host0, int has_common, int w, AsmItem *items, int *list) {
@@ -495,8 +522,9 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
       for (int k = 0; k < p.num_landmarks; k++) { fp[k] = run; while (i < p.num_vis && vl[i] == k) { i++; run++; } h.lm_win[m.lm_off + k] = w; } }
     // assembly plan
     // frame-pair order of the X records (counting sort by (host, observer); the one-frame factors of WIDE records form the "pair" (host, host)),
-    // pair chunks; for the solver (all factors) and for the marginalisation of frame 0 (the factors hosted there)
-    auto pair_tables = [&](bool marg, int *vp, AsmItem *pit, int base, int wide) {
+    // pair chunks; for the solver (all factors) and for the marginalisation of frame 0 (the factors hosted there).  vp: each factor's record slot
+    // (nullptr: compact solver windows, whose records are never stored); first_item: per pair (host * NFR + observer) its first chunk, -1: none
+    auto pair_tables = [&](bool marg, int *vp, AsmItem *pit, int base, int wide, int *first_item) {
         int pcnt[NFR * NFR] = {0}, poff[NFR * NFR];
         for (int i = 0; i < p.num_vis; i++) {
             if (marg && vi[i] != 0) continue;
@@ -505,25 +533,46 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
         int pos = 0, ni = 0;
         for (int a = 0; a < NFR * NFR; a++) {
             poff[a] = pos;
+            first_item[a] = pcnt[a] ? ni : -1;
             for (int c0 = 0, ph = 0; c0 < pcnt[a]; c0 += PAIR_CHUNK, ph++) {
                 AsmItem &it = pit[ni++];
                 it.kind = ITEM_PAIR; it.win = w; it.a = a / NFR; it.b = a % NFR; it.lo = pos + c0; it.hi = pos + std::min(pcnt[a], c0 + (int)PAIR_CHUNK); it.phase = ph; it.has_common = wide; it.base = base;
             }
             pos += pcnt[a];
         }
-        for (int i = 0; i < p.num_vis; i++) {
+        if (vp) for (int i = 0; i < p.num_vis; i++) {
             if (marg && vi[i] != 0) { vp[i] = -1; continue; }
             if (vt[i] != 2) vp[i] = poff[vi[i] * NFR + vj[i]]++; else if (wide) vp[i] = poff[vi[i] * NFR + vi[i]]++; else vp[i] = -1;
         }
     };
-    if (m.fused) pair_tables(false, h.vis_pos + m.vis_off, h.pitems + m.pitem_off, m.xrec_off, m.has_common);
-    if (m.mfused) pair_tables(true, h.mvis_pos + m.vis_off, h.mpitems + m.mpitem_off, m.mxrec_off, 1);
-    if (m.fused || m.mfused) {
-        // duplicate codes (two factors of one landmark observed from the same frame: left and right camera, consecutive), landmark blocks
+    int pfirst[NFR * NFR];
+    if (m.fused) pair_tables(false, m.has_common ? h.vis_pos + m.vis_off : nullptr, h.pitems + m.pitem_off, m.xrec_off, m.has_common, pfirst);
+    if (m.fused && !m.has_common) {      // host runs: descriptors (at their slot in the longest-first order), tiles, factor and landmark lists in run order
+        int *rf = h.run_f + m.vis_off, *rl = h.run_lm + 2 * (size_t)m.lm_off;
+        RunTile *rt = h.run_tile + lo.rtile_off;
+        int nfac = 0, nlmk = 0, ntl = 0, cur = -1;
+        host_runs(p.num_vis, vl, vi, p.num_landmarks, [&](int hf, int k, int first, int cnt, bool fresh) {
+            if (hf != cur) {
+                RunDesc &d = h.run_desc[lo.run_slot[hf]]; memset(&d, 0, sizeof d);
+                d.win = w; d.host = hf; d.t0 = lo.rtile_off + ntl; d.ntile = lo.run_nt[hf];
+                for (int j = 0; j < NFR; j++) d.pfirst[j] = pfirst[hf * NFR + j] >= 0 ? m.pitem_off + pfirst[hf * NFR + j] : -1;
+                cur = hf;
+            }
+            if (fresh) { RunTile &t = rt[ntl++]; t.l0 = m.lm_off + nlmk; t.nl = 0; t.f0 = m.vis_off + nfac; t.nf = 0; }
+            RunTile &t = rt[ntl - 1];
+            rl[2 * nlmk] = m.lm_off + k; rl[2 * nlmk + 1] = t.nf; nlmk++; t.nl++;
+            for (int q = 0; q < cnt; q++) rf[nfac++] = m.vis_off + first + q;
+            t.nf += cnt;
+        });
+    }
+    if (m.mfused) pair_tables(true, h.mvis_pos + m.vis_off, h.mpitems + m.mpitem_off, m.mxrec_off, 1, pfirst);
+    if (m.fused || m.mfused) {      // duplicate codes (two factors of one landmark observed from the same frame: left and right camera, consecutive)
         for (int i = 0; i < p.num_vis; i++) {
             if (vt[i] == 2) continue;
             if (i > 0 && vt[i - 1] != 2 && vl[i - 1] == vl[i] && vj[i - 1] == vj[i]) { vd[i - 1] = 1; vd[i] = 2; }
         }
+    }
+    if (lo.nlmb > 0) {      // landmark blocks of lin_vis_lm_wide
         LmbDesc *ld = h.lmb_desc + m.lmb_off;
         int nb = 0, in_blk = 0, i = 0; bool open = false;
         for (int k = 0; k < p.num_landmarks; k++) {
@@ -599,9 +648,25 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
         b->meta[w].fused = fused ? 1 : 0; b->meta[w].mfused = mfused ? 1 : 0;
         if (fused) { low[w].nitems_s = 0; low[w].nlist_s = 0; low[w].nph_s = 0; b->meta[w].nitems = 0; b->meta[w].nphases = 0; if (b->meta[w].has_common) n_fused_wide++; else n_fused_compact++; }
         else { low[w].npitems = 0; low[w].nxrec = 0; n_unfused++; }
+        if (!fused || b->meta[w].has_common) { low[w].nrun = 0; low[w].nrtile = 0; }
         if (mfused) { low[w].nitems_m = 0; low[w].nlist_m = 0; low[w].nph_m = 0; b->meta[w].nmitems = 0; b->meta[w].nmphases = 0; n_mfused++; }
         else { low[w].nmpitems = 0; low[w].nmxrec = 0; if (b->meta[w].margin_flag == 0) n_munfused++; }
-        if (!fused && !mfused) low[w].nlmb = 0;
+        if (!(fused && b->meta[w].has_common) && !mfused) low[w].nlmb = 0;
+    }
+    // host runs, longest first (a counting sort by tile count): every window's long run (its frame-0 run, on the bench's windows) starts in the first
+    // waves instead of forming the tail
+    size_t nrun = 0, nrtile = 0;
+    {
+        int maxt = 0;
+        for (int w = 0; w < B; w++) for (int f = 0; f < NFR; f++) maxt = std::max(maxt, low[w].nrun ? low[w].run_nt[f] : 0);
+        std::vector<size_t> start((size_t)maxt + 2, 0);
+        for (int w = 0; w < B; w++) if (low[w].nrun) for (int f = 0; f < NFR; f++) if (low[w].run_nt[f]) start[maxt - low[w].run_nt[f] + 1]++;
+        for (int t = 1; t <= maxt + 1; t++) start[t] += start[t - 1];
+        for (int w = 0; w < B; w++) {
+            WinLow &lo = low[w];
+            lo.rtile_off = (int)nrtile; nrtile += lo.nrtile; nrun += lo.nrun;
+            if (lo.nrun) for (int f = 0; f < NFR; f++) if (lo.run_nt[f]) lo.run_slot[f] = (int)start[maxt - lo.run_nt[f]]++;
+        }
     }
     // ---- phase 2: offsets
     size_t nlmb = 0, npit = 0, nxr = 0, nmpit = 0, nmxr = 0;      // nxr / nmxr: record regions in DOUBLES (solver / marginalisation share one buffer)
@@ -636,7 +701,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     bd.nvis_total = (int)nvis; bd.nlm_total = (int)nlm; bd.nimu_total = (int)nimu; bd.nwheel_total = (int)nwheel; bd.nplane_total = (int)nplane; bd.nprior = (int)npri;
     bd.nitems_solve = (int)nit_s; bd.nitems_marg = (int)nit_m;
     bd.rec_stride_solve = VREC_COMPACT;
-    bd.n_unfused = n_unfused; bd.nlmb_total = (int)nlmb; bd.npitems_total = (int)npit; bd.nmpitems_total = (int)nmpit;
+    bd.n_unfused = n_unfused; bd.nlmb_total = (int)nlmb; bd.npitems_total = (int)npit; bd.nmpitems_total = (int)nmpit; bd.nrun_total = (int)nrun;
     bd.pitems_max = 1; for (int w = 0; w < B; w++) bd.pitems_max = std::max(bd.pitems_max, std::max(b->meta[w].npitems, b->meta[w].nmpitems));
     {   // pair_win keeps a window's chunk products in shared memory: possible when the largest window fits next to a second resident block
         size_t need_s = 0, need_m = 0;
@@ -646,7 +711,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
             if (mw.mfused) need_m = std::max(need_m, pair_win_smem_bytes(mw.nmpitems, (int)XL<true>::OUT));
         }
         const size_t cap = 110 * 1024;
-        bd.pwin_smem = (!g_no_pair_win && need_s > 0 && need_s <= cap) ? (int)need_s : 0;
+        bd.pwin_smem = (!g_no_pair_win && n_fused_compact == 0 && need_s > 0 && need_s <= cap) ? (int)need_s : 0;
         bd.pwin_smem_marg = (!g_no_pair_win && need_m > 0 && need_m <= cap) ? (int)need_m : 0;
     }
     bd.n_fused_wide = n_fused_wide; bd.n_fused_compact = n_fused_compact; bd.n_mfused = n_mfused; bd.n_munfused = n_munfused;
@@ -665,8 +730,9 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     IN(&bd.imu_fi, nimu); IN(&bd.imu_fj, nimu); IN(&bd.imu_win, nimu); IN(&bd.wheel_fi, nwheel); IN(&bd.wheel_fj, nwheel); IN(&bd.wheel_win, nwheel);
     IN(&bd.plane_f, nplane); IN(&bd.plane_win, nplane); IN(&bd.imu_data, nimu * 287); IN(&bd.wheel_data, nwheel * 78);
     IN(&bd.prior_J, npJ); IN(&bd.prior_r, npr); IN(&bd.prior_x0, npri * SFIX); IN(&bd.x_init, nstate); IN(&b->work_init_dev, B);
-    IN(&bd.vis_pos, npit ? nvis : 0); IN(&bd.lmb_desc, nlmb); IN(&bd.pitems, npit);
+    IN(&bd.vis_pos, n_fused_wide ? nvis : 0); IN(&bd.lmb_desc, nlmb); IN(&bd.pitems, npit);
     IN(&bd.mvis_pos, nmpit ? nvis : 0); IN(&bd.mpitems, nmpit);
+    IN(&bd.run_desc, nrun); IN(&bd.run_tile, nrtile); IN(&bd.run_f, nrun ? nvis : 0); IN(&bd.run_lm, nrun ? 2 * nlm : 0);
     const size_t nvec = (size_t)B * TFIX + nlm;
     WK(&bd.work, B); WK(&bd.x_cur, nstate); WK(&bd.x_cand, nstate); WK(&bd.x_before, nstate);
     WK(&bd.vis_type, nvis); WK(&bd.vis_fi, nvis); WK(&bd.vis_fj, nvis); WK(&bd.vis_win, nvis); WK(&bd.vis_dup, nvis); WK(&bd.vis_obs, nvis * 12);
@@ -703,7 +769,8 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
       HP(h.meta); HP(h.prior); HP(h.vis_code); HP(h.vis_lm); HP(h.vis_oi); HP(h.obs_i); HP(h.obs_j); HP(h.lm_win); HP(h.lm_fptr); HP(h.items); HP(h.asm_list);
       HP(h.imu_fi); HP(h.imu_fj); HP(h.imu_win); HP(h.wheel_fi); HP(h.wheel_fj); HP(h.wheel_win); HP(h.plane_f); HP(h.plane_win); HP(h.imu_data); HP(h.wheel_data);
       HP(h.prior_J); HP(h.prior_r); HP(h.prior_x0); HP(h.x_init); HP(h.work);
-      HP(h.vis_pos); HP(h.lmb_desc); HP(h.pitems); HP(h.mvis_pos); HP(h.mpitems); }
+      HP(h.vis_pos); HP(h.lmb_desc); HP(h.pitems); HP(h.mvis_pos); HP(h.mpitems);
+      HP(h.run_desc); HP(h.run_tile); HP(h.run_f); HP(h.run_lm); }
     h.nitems_solve_total = (int)nit_s;
     for (auto &e : ents) *e.field = ar->dev + e.off;
     if (npri) memcpy(h.prior, priors.data(), sizeof(PriorDev) * npri);
@@ -731,6 +798,7 @@ static int ensure_attrs(viwb_context *ctx) {
     if (!ctx->attrs_set) {
         CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_NT, TFIX * (TFIX + 1) / 2) * 8)));
         CK(cudaFuncSetAttribute(lin_vis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_smem_doubles(128, VREC) * 8)));
+        CK(cudaFuncSetAttribute(lin_vis_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_run_smem_doubles() * 8)));
         CK(cudaFuncSetAttribute(lin_vis_lm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_lm_smem_doubles(true) * 8)));
         CK(cudaFuncSetAttribute(syrk_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(syrk_mma_smem_doubles() * 8)));
         CK(cudaFuncSetAttribute(pair_win_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
@@ -769,14 +837,13 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
         const int nfi = solve ? bd.npitems_total : bd.nmpitems_total;               // fused pair items of this mode
         if (solve) {
             const int vmode = cost_only ? (int)MODE_COST : mode;
-            if (bd.n_fused_compact > 0) { LAUNCH(lin_vis_lm, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(false) * 8, vmode, st); ctx->launches++; }
+            if (bd.n_fused_compact > 0) { LAUNCH(lin_vis_lm, bd, bd.nrun_total, 1, NT(LMB_FACTORS), lin_vis_run_smem_doubles() * 8, vmode, st); ctx->launches++; }      // + the compact windows' pair chunks
             if (bd.n_fused_wide > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, vmode, st); ctx->launches++; }
         } else if (bd.n_mfused > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, mode, st); ctx->launches++; }
         auto fused_asm = [&]() {
             if (nfi <= 0) return;
             const int pw = solve ? bd.pwin_smem : bd.pwin_smem_marg;
             if (pw > 0) { LAUNCH(pair_win, bd, B, 1, NT(256), (size_t)pw, mode, st); ctx->launches++; return; }
-            if (solve && bd.n_fused_compact > 0) { LAUNCH(asm_pairs, bd, (nfi + wpb2 - 1) / wpb2, 1, NT(128), 0, mode, st); ctx->launches++; }
             if (!solve || bd.n_fused_wide > 0) { LAUNCH(asm_pairs_wide, bd, (nfi + wpb2 - 1) / wpb2, 1, NT(128), 0, mode, st); ctx->launches++; }
             LAUNCH(pair_reduce, bd, B, 1, NT(PAIR_RED_NT), (size_t)bd.pitems_max * sizeof(int), mode, st); ctx->launches++;
         };
