@@ -3,7 +3,8 @@
 // HBM layout (all FP64 unless noted; B windows, concatenated):
 //   x_cur / x_cand      [sum(207 + nlm)]        parameter blocks, fixed-state layout of include/viwb.h + inverse depths
 //   vis_*               visual factor table, sorted by landmark; vis_obs stays [nvis][12] as given
-//   vis_rec             [nvis_total][28 or 54]  per-factor record written by lin_vis: r(2) A(12) B(12) Jl(2) | Jtd(2) E0(12) E1(12)
+//   vis_rec             [nvis_total][28 or 54]  per-factor record written by lin_vis: r(2) A(12) B(12) Jl(2) | Jtd(2) E0(12) E1(12); like vis_cost
+//                       only allocated when some window's solve or marginalisation takes the unfused path
 //   lm_*                per landmark: a = |J_l|^2, gl = J_l^T r, gamma = c^2/h (Schur weight), W [80] = J_p^T J_l over the
 //                       "visual subspace" (11 poses x 6 | ex0 6 | ex1 6 | td 1 | pad)
 //   imu_rec / wheel_rec / plane_rec   whitened residual + tangent Jacobian of the small factors
@@ -141,8 +142,8 @@ struct BatchDev {       // passed by value to every kernel
     // observation (pts_j, velocity_j, td_j) and an index into the table of host sides (pts_i, velocity_i, td_i), which every factor of a landmark shares
     const int *vis_code, *vis_oi;
     const double *obs_i, *obs_j;    // [nobs_i_total][6], [nvis_total][6]
-    double *vis_rec;                // [nvis_total][VREC]
-    double *vis_cost;               // [nvis_total]
+    double *vis_rec;                // [nvis_total][VREC] if some window is unfused (n_unfused or n_munfused), else a placeholder
+    double *vis_cost;               // [nvis_total] the same
     // assembly plan (static per batch): items = chunks of per-frame / per-frame-pair / common factor lists
     const struct AsmItem *items;    // solver items of all windows, then marginalisation items
     const int *asm_list;            // list entries: (window-local factor index << 1) | role; item.lo/hi are relative to meta.list_off / mlist_off

@@ -236,19 +236,20 @@ static double window_algorithmic_bytes(const viwb_problem &p, int iters) {
 
 static void batch_free(viwb_context *ctx, viwb_batch *b);
 
-// ---- per-window lowering, phase 1: validation, sizes, active columns, marginalisation plan (no offsets yet)
+// ---- per-window lowering, phase 1: validation, sizes, active columns, and the plan (no offsets yet): the paths of the window's solver linearisation
+// and marginalisation, and the sizes of those paths' tables only (the ones the kernels read in WinMeta: nitems, npitems, nlmb, ...)
+enum SolvePath { SOLVE_UNFUSED, SOLVE_COMPACT, SOLVE_WIDE };      // lin_vis + lm_reduce + asm_items; host runs of lin_vis_lm; landmark blocks of lin_vis_lm_wide + asm_pairs_wide
+enum MargPath { MARG_NONE, MARG_UNFUSED, MARG_WIDE };             // none: no visual factor is marginalised (window not full, no flag, or MARGIN_SECOND_NEW)
 struct WinLow {
     int err; bool grouped, has_prior;
-    int nlist_s, nitems_s, nph_s, nlist_m, nitems_m, nph_m;
     int prior_n_out;
-    bool regular;               // fused path possible: grouped table, <= LMB_FACTORS factors per landmark, at most two factors per (landmark, observer), consecutive
-    int nlmb, npitems, nxrec;   // landmark blocks of lin_vis_lm_wide, pair chunks, wide records (two-frame factors + the one-frame ones)
-    int nrun, nrtile, rtile_off;              // compact windows: host runs of lin_vis_lm, their tiles, the first tile's index
-    int run_nt[NFR], run_slot[NFR];           // per host frame: tiles of its run, the run's descriptor index (runs are ordered longest first)
-    int nmpitems, nmxrec;       // the same for the marginalisation of frame 0 (factors hosted there, wide records)
     bool obs_per_factor; int nobs_i, obsi_off;       // entries of the host-side observation table (wire format): one per run of factors with an identical (pts_i, velocity_i, td_i)
+    int solve, marg;                                  // SolvePath, MargPath
+    int nlist_s, nlist_m;                             // unfused solve / marginalisation: gather-list entries (emit_lists)
+    int nrun, nrtile, rtile_off;                      // compact solve: host runs of lin_vis_lm, their tiles, the first tile's index
+    int run_nt[NFR], run_slot[NFR];                   // per host frame: tiles of its run, the run's descriptor index (runs are ordered longest first)
 };
-static int chunk_count(int n) { return (n + ASM_CHUNK - 1) / ASM_CHUNK; }
+static int chunk_count(int n, int chunk = ASM_CHUNK) { return (n + chunk - 1) / chunk; }
 // columns of a visual factor's 12-double observation record (viwb.h): pts_i (0..2) pts_j (3..5) velocity_i (6,7) velocity_j (8,9) td_i (10) td_j (11)
 static inline bool same_host_side(const double *a, const double *b) {      // bitwise (the wire format must reproduce the caller's table exactly)
     auto bits = [](const double *p) { unsigned long long v; memcpy(&v, p, sizeof v); return v; };
@@ -277,7 +278,7 @@ template <typename F> static void host_runs(int nvis, const int *vl, const int *
     }
 }
 
-static void lower_count(const viwb_problem &p, int mf, WinMeta &m, WinLow &lo, int &out_mode) {
+static void lower_count(const viwb_problem &p, int mf, bool allow_fused, WinMeta &m, WinLow &lo, int &out_mode) {
     memset(&m, 0, sizeof m); memset(&lo, 0, sizeof lo);
     if (p.frame_count < 0 || p.frame_count > VIWB_WINDOW_SIZE || p.num_landmarks < 0 || p.num_landmarks > VIWB_MAX_LANDMARKS) { lo.err = 1; return; }
     if (p.num_vis < 0 || p.num_imu < 0 || p.num_wheel < 0 || p.num_plane < 0) { lo.err = 5; return; }            // counts are added up as size_t below
@@ -387,61 +388,60 @@ static void lower_count(const viwb_problem &p, int mf, WinMeta &m, WinLow &lo, i
             lo.prior_n_out = nn;
         }
     }
-    // assembly plan sizes
-    int nframe_ent = 0, npair_ent = 0;
-    for (int a = 0; a < NFR; a++) { nframe_ent += fcnt[a]; lo.nitems_s += chunk_count(fcnt[a]); lo.nph_s = std::max(lo.nph_s, chunk_count(fcnt[a])); }
-    for (int a = 0; a < NFR * NFR; a++) { npair_ent += pcnt[a]; lo.nitems_s += chunk_count(pcnt[a]); lo.nph_s = std::max(lo.nph_s, chunk_count(pcnt[a])); }
-    lo.nlist_s = nframe_ent + npair_ent;
-    if (m.has_common) { lo.nlist_s += p.num_vis; lo.nitems_s += chunk_count(p.num_vis); lo.nph_s = std::max(lo.nph_s, chunk_count(p.num_vis)); }
-    if (m.margin_flag == 0) {
-        for (int a = 0; a < NFR; a++) { lo.nlist_m += fcnt0[a]; lo.nitems_m += chunk_count(fcnt0[a]); lo.nph_m = std::max(lo.nph_m, chunk_count(fcnt0[a])); }
-        for (int a = 0; a < NFR * NFR; a++) { lo.nlist_m += pcnt0[a]; lo.nitems_m += chunk_count(pcnt0[a]); lo.nph_m = std::max(lo.nph_m, chunk_count(pcnt0[a])); }
-        lo.nlist_m += ncommon0; lo.nitems_m += chunk_count(ncommon0); lo.nph_m = std::max(lo.nph_m, chunk_count(ncommon0));
-    }
-    m.nitems = lo.nitems_s; m.nphases = lo.nph_s; m.nmitems = lo.nitems_m; m.nmphases = lo.nph_m;
-    // fused-path plan (kernels_fused.cuh): sizes only; lower_fill builds the tables
     // wire format: runs of factors sharing one host-side observation (a grouped table: one run per landmark, estimator.cpp:1595-1597 takes
     // pts_i / velocity_i / td_i from the landmark's first observation for every factor); an ungrouped table keeps one entry per factor
     // (assumed here -- the plan never reads the observations --, verified when lower_fill copies them; a table that breaks it is rebuilt with one entry per factor)
     lo.obs_per_factor = !lo.grouped; lo.nobs_i = lo.grouped ? p.num_landmarks : p.num_vis;
-    lo.regular = lo.grouped;
-    lo.nxrec = 0; lo.npitems = 0; lo.nlmb = 0; lo.nmxrec = 0; lo.nmpitems = 0;
-    for (int a = 0; a < NFR * NFR; a++) { lo.nxrec += pcnt[a]; lo.npitems += (pcnt[a] + PAIR_CHUNK - 1) / PAIR_CHUNK; }
-    if (m.has_common) {      // wide records: the one-frame factors carry ex0 / ex1 / td columns; they form the "pairs" (host, host), one group per host frame
-        int scnt[NFR] = {0};
-        for (int i = 0; i < p.num_vis; i++) if (p.vis_type[i] == 2) scnt[p.vis_frame_i[i]]++;
-        for (int a = 0; a < NFR; a++) { lo.nxrec += scnt[a]; lo.npitems += (scnt[a] + PAIR_CHUNK - 1) / PAIR_CHUNK; }
-    }
-    if (m.margin_flag == 0) {
-        int two = 0;
-        for (int a = 0; a < NFR * NFR; a++) { two += pcnt0[a]; lo.nmpitems += (pcnt0[a] + PAIR_CHUNK - 1) / PAIR_CHUNK; }
-        lo.nmxrec = ncommon0; lo.nmpitems += (ncommon0 - two + PAIR_CHUNK - 1) / PAIR_CHUNK;
-    }
-    if (lo.regular) {
-        int in_blk = 0, i = 0; bool open = false;
-        for (int k = 0; k < p.num_landmarks && lo.regular; k++) {
-            int cnt = 0, seenj[NFR], ndup[NFR];
-            for (int q = 0; q < NFR; q++) { seenj[q] = -2; ndup[q] = 0; }
-            for (; i < p.num_vis && p.vis_landmark[i] == k; i++, cnt++) {
-                if (p.vis_type[i] == 2) continue;
-                const int fj = p.vis_frame_j[i];
-                if (ndup[fj] == 0) { ndup[fj] = 1; seenj[fj] = i; }
-                else if (ndup[fj] == 1 && seenj[fj] == i - 1) ndup[fj] = 2;
-                else lo.regular = false;
-            }
-            if (cnt > LMB_FACTORS) lo.regular = false;
-            if (!open || in_blk + cnt > LMB_FACTORS) { lo.nlmb++; in_blk = 0; open = true; }
-            in_blk += cnt;
+    // the paths (kernels_fused.cuh).  A regular table -- grouped, <= LMB_FACTORS factors per landmark, at most two factors per (landmark, observer),
+    // consecutive -- takes the fused path where it has pair chunks: compact records (host runs) unless ex0 / ex1 / td are active, wide records
+    // otherwise; the marginalisation of frame 0 always takes wide records.  Decided per window, so that a window takes the same path -- and gives
+    // the same bits -- whatever else the batch holds.  nlmb: landmark blocks of lin_vis_lm_wide (whole landmarks, <= LMB_FACTORS factors)
+    bool regular = lo.grouped;
+    int nlmb = 0;
+    for (int k = 0, i = 0, in_blk = 0; k < p.num_landmarks && regular; k++) {
+        int cnt = 0, seenj[NFR], ndup[NFR];
+        for (int q = 0; q < NFR; q++) { seenj[q] = -2; ndup[q] = 0; }
+        for (; i < p.num_vis && p.vis_landmark[i] == k; i++, cnt++) {
+            if (p.vis_type[i] == 2) continue;
+            const int fj = p.vis_frame_j[i];
+            if (ndup[fj] == 0) { ndup[fj] = 1; seenj[fj] = i; }
+            else if (ndup[fj] == 1 && seenj[fj] == i - 1) ndup[fj] = 2;
+            else regular = false;
         }
+        if (cnt > LMB_FACTORS) regular = false;
+        if (k == 0 || in_blk + cnt > LMB_FACTORS) { nlmb++; in_blk = 0; }
+        in_blk += cnt;
     }
-    if (lo.regular && !m.has_common) {      // compact records: the pairs' products are formed per host run, no record is stored
-        lo.nxrec = 0;
+    // pair chunks: one group per frame pair; with wide records the one-frame factors (which carry ex0 / ex1 / td columns) form the "pairs" (host, host)
+    int npit = 0, nmpit = 0, nxrec = 0, two0 = 0, scnt[NFR] = {0};
+    if (m.has_common) for (int i = 0; i < p.num_vis; i++) if (p.vis_type[i] == 2) scnt[p.vis_frame_i[i]]++;
+    for (int a = 0; a < NFR * NFR; a++) { nxrec += pcnt[a]; npit += chunk_count(pcnt[a], PAIR_CHUNK); two0 += pcnt0[a]; nmpit += chunk_count(pcnt0[a], PAIR_CHUNK); }
+    for (int a = 0; a < NFR; a++) { nxrec += scnt[a]; npit += chunk_count(scnt[a], PAIR_CHUNK); }
+    nmpit += chunk_count(ncommon0 - two0, PAIR_CHUNK);
+    const bool fused = allow_fused && regular && npit > 0, mfused = allow_fused && regular && m.margin_flag == 0 && nmpit > 0;
+    lo.solve = !fused ? SOLVE_UNFUSED : m.has_common ? SOLVE_WIDE : SOLVE_COMPACT;
+    lo.marg = m.margin_flag != 0 ? MARG_NONE : mfused ? MARG_WIDE : MARG_UNFUSED;
+    m.fused = fused; m.mfused = mfused;
+    // the sizes of the chosen paths' tables; lower_fill builds them
+    auto list_sizes = [](const int *fc, const int *pc, int ncom, int &nlist, int &nitems, int &nphases) {      // emit_lists: frame lists, pair lists, common list
+        auto add = [&](int n) { nlist += n; nitems += chunk_count(n); nphases = std::max(nphases, chunk_count(n)); };
+        for (int a = 0; a < NFR; a++) add(fc[a]);
+        for (int a = 0; a < NFR * NFR; a++) add(pc[a]);
+        add(ncom);
+    };
+    if (lo.solve == SOLVE_UNFUSED) list_sizes(fcnt, pcnt, m.has_common ? p.num_vis : 0, lo.nlist_s, m.nitems, m.nphases);
+    if (lo.solve == SOLVE_COMPACT) {      // the pairs' products are formed per host run, no record is stored
+        m.npitems = npit;
         host_runs(p.num_vis, p.vis_landmark, p.vis_frame_i, p.num_landmarks, [&](int h, int, int, int, bool fresh) { if (fresh) { if (lo.run_nt[h]++ == 0) lo.nrun++; lo.nrtile++; } });
     }
+    if (lo.solve == SOLVE_WIDE) { m.npitems = npit; m.nxrec = nxrec; }
+    if (lo.marg == MARG_UNFUSED) list_sizes(fcnt0, pcnt0, ncommon0, lo.nlist_m, m.nmitems, m.nmphases);
+    if (lo.marg == MARG_WIDE) { m.nmpitems = nmpit; m.nmxrec = ncommon0; }
+    if (lo.solve == SOLVE_WIDE || lo.marg == MARG_WIDE) m.nlmb = nlmb;
 }
 
 // ---- phase 3: fill this window's slices of the (pinned) staging arrays; every offset is final
-struct HostArrays {
+struct HostArrays {      // the input arrays' views in the staging slab (batch_build's slab table sets them)
     WinMeta *meta; PriorDev *prior; int *vis_code, *vis_lm, *vis_oi; double *obs_i, *obs_j; int *lm_win, *lm_fptr;
     AsmItem *items; int *asm_list; int *imu_fi, *imu_fj, *imu_win, *wheel_fi, *wheel_fj, *wheel_win, *plane_f, *plane_win;
     double *imu_data, *wheel_data, *prior_J, *prior_r, *prior_x0, *x_init; WinWork *work;
@@ -520,8 +520,8 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
     // landmark -> factor ranges (global factor indices)
     { int *fp = h.lm_fptr + m.lm_off; int run = m.vis_off, i = 0;
       for (int k = 0; k < p.num_landmarks; k++) { fp[k] = run; while (i < p.num_vis && vl[i] == k) { i++; run++; } h.lm_win[m.lm_off + k] = w; } }
-    // assembly plan
-    // frame-pair order of the X records (counting sort by (host, observer); the one-frame factors of WIDE records form the "pair" (host, host)),
+    // the tables of the window's paths (lower_count sized exactly these)
+    // pair_tables: frame-pair order of the X records (counting sort by (host, observer); the one-frame factors of WIDE records form the "pair" (host, host)),
     // pair chunks; for the solver (all factors) and for the marginalisation of frame 0 (the factors hosted there).  vp: each factor's record slot
     // (nullptr: compact solver windows, whose records are never stored); first_item: per pair (host * NFR + observer) its first chunk, -1: none
     auto pair_tables = [&](bool marg, int *vp, AsmItem *pit, int base, int wide, int *first_item) {
@@ -545,9 +545,22 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
             if (vt[i] != 2) vp[i] = poff[vi[i] * NFR + vj[i]]++; else if (wide) vp[i] = poff[vi[i] * NFR + vi[i]]++; else vp[i] = -1;
         }
     };
+    auto landmark_table = [&]() {      // landmark blocks of lin_vis_lm_wide (the wide solve and the wide marginalisation share them)
+        LmbDesc *ld = h.lmb_desc + m.lmb_off;
+        for (int k = 0, i = 0, nb = 0; k < p.num_landmarks; k++) {
+            const int first = i;
+            while (i < p.num_vis && vl[i] == k) i++;
+            if (k == 0 || ld[nb - 1].nf + (i - first) > LMB_FACTORS) { LmbDesc &d = ld[nb++]; memset(&d, 0, sizeof d); d.win = w; d.k0 = m.lm_off + k; d.f0 = m.vis_off + first; }
+            ld[nb - 1].k1 = m.lm_off + k + 1;           // the open block ends after this landmark
+            ld[nb - 1].nf += i - first;
+        }
+    };
     int pfirst[NFR * NFR];
-    if (m.fused) pair_tables(false, m.has_common ? h.vis_pos + m.vis_off : nullptr, h.pitems + m.pitem_off, m.xrec_off, m.has_common, pfirst);
-    if (m.fused && !m.has_common) {      // host runs: descriptors (at their slot in the longest-first order), tiles, factor and landmark lists in run order
+    switch (lo.solve) {
+    case SOLVE_UNFUSED: emit_lists(vt, vi, vj, p.num_vis, false, m.has_common, w, h.items + m.item_off, h.asm_list + m.list_off); break;
+    case SOLVE_WIDE: pair_tables(false, h.vis_pos + m.vis_off, h.pitems + m.pitem_off, m.xrec_off, 1, pfirst); landmark_table(); break;
+    case SOLVE_COMPACT: {      // pair chunks without records; host runs: descriptors (at their slot in the longest-first order), tiles, factor and landmark lists in run order
+        pair_tables(false, nullptr, h.pitems + m.pitem_off, m.xrec_off, 0, pfirst);
         int *rf = h.run_f + m.vis_off, *rl = h.run_lm + 2 * (size_t)m.lm_off;
         RunTile *rt = h.run_tile + lo.rtile_off;
         int nfac = 0, nlmk = 0, ntl = 0, cur = -1;
@@ -564,30 +577,20 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
             for (int q = 0; q < cnt; q++) rf[nfac++] = m.vis_off + first + q;
             t.nf += cnt;
         });
+        break;
     }
-    if (m.mfused) pair_tables(true, h.mvis_pos + m.vis_off, h.mpitems + m.mpitem_off, m.mxrec_off, 1, pfirst);
+    }
+    switch (lo.marg) {      // (MARG_NONE: no table)
+    case MARG_UNFUSED: emit_lists(vt, vi, vj, p.num_vis, true, 1, w, h.items + h.nitems_solve_total + m.mitem_off, h.asm_list + m.mlist_off); break;
+    case MARG_WIDE: pair_tables(true, h.mvis_pos + m.vis_off, h.mpitems + m.mpitem_off, m.mxrec_off, 1, pfirst); if (lo.solve != SOLVE_WIDE) landmark_table(); break;
+    }
     if (m.fused || m.mfused) {      // duplicate codes (two factors of one landmark observed from the same frame: left and right camera, consecutive)
         for (int i = 0; i < p.num_vis; i++) {
             if (vt[i] == 2) continue;
             if (i > 0 && vt[i - 1] != 2 && vl[i - 1] == vl[i] && vj[i - 1] == vj[i]) { vd[i - 1] = 1; vd[i] = 2; }
         }
     }
-    if (lo.nlmb > 0) {      // landmark blocks of lin_vis_lm_wide
-        LmbDesc *ld = h.lmb_desc + m.lmb_off;
-        int nb = 0, in_blk = 0, i = 0; bool open = false;
-        for (int k = 0; k < p.num_landmarks; k++) {
-            const int first = i;
-            int cnt = 0;
-            for (; i < p.num_vis && vl[i] == k; i++) cnt++;
-            if (!open || in_blk + cnt > LMB_FACTORS) { LmbDesc &d = ld[nb++]; memset(&d, 0, sizeof d); d.win = w; d.k0 = m.lm_off + k; d.f0 = m.vis_off + first; in_blk = 0; open = true; }
-            ld[nb - 1].k1 = m.lm_off + k + 1;           // the open block ends after this landmark
-            in_blk += cnt; ld[nb - 1].nf = in_blk;
-        }
-    }
     { int *vc = h.vis_code + m.vis_off; for (int i = 0; i < p.num_vis; i++) vc[i] = vt[i] | (vi[i] << 2) | (vj[i] << 6) | ((int)vd[i] << 10); }
-    if (!m.fused)
-    emit_lists(vt, vi, vj, p.num_vis, false, m.has_common, w, h.items + m.item_off, h.asm_list + m.list_off);
-    if (m.margin_flag == 0 && !m.mfused) emit_lists(vt, vi, vj, p.num_vis, true, 1, w, h.items + h.nitems_solve_total + m.mitem_off, h.asm_list + m.mlist_off);
 
     // small factors
     for (int i = 0; i < p.num_imu; i++) { h.imu_fi[m.imu_off + i] = p.imu_frame_i[i]; h.imu_fj[m.imu_off + i] = p.imu_frame_j[i]; h.imu_win[m.imu_off + i] = w; }
@@ -634,38 +637,28 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     b->meta.resize(B); b->out_mode.assign(B, 2); b->in_prior.resize(B); b->state_sizes.resize(B); b->prior_n.assign(B, 0);
     std::vector<WinLow> low(B);
     // ---- phase 1 (parallel): sizes and plans
-    parallel_for(B, [&](int w) { lower_count(problems[w], margin_flags ? margin_flags[w] : -1, b->meta[w], low[w], b->out_mode[w]); });
+    const bool allow_fused = getenv("VIWB_NO_FUSED") == nullptr;      // read once per build: every window of the batch is planned under the same switch
+    parallel_for(B, [&](int w) { lower_count(problems[w], margin_flags ? margin_flags[w] : -1, allow_fused, b->meta[w], low[w], b->out_mode[w]); });
     const double t_counted = now_ms();
     if (obs_per_factor) for (int w = 0; w < B; w++) { low[w].obs_per_factor = true; low[w].nobs_i = problems[w].num_vis < 0 ? 0 : problems[w].num_vis; }
     for (int w = 0; w < B; w++) if (low[w].err) { const int e = low[w].err; batch_free(ctx, b); return fail(ctx, VIWB_ERR_INVALID, e == 1 ? "bad frame_count / num_landmarks" : e == 2 ? "bad prior" : e == 3 ? "bad visual factor table" : e == 5 ? "negative factor count or missing table" : "bad factor frame index"); }
-    // fused solver linearisation (kernels_fused.cuh) when every window qualifies; then the solver's gather lists are not built at all
-    // (decided per window, so that a window takes the same path -- and gives the same bits -- whatever else the batch holds)
-    const bool allow_fused = getenv("VIWB_NO_FUSED") == nullptr;
-    int n_unfused = 0, n_fused_wide = 0, n_fused_compact = 0, n_mfused = 0, n_munfused = 0;
-    for (int w = 0; w < B; w++) {
-        const bool fused = allow_fused && low[w].regular && low[w].npitems > 0;      // (a window without two-frame factors has nothing to fuse)
-        const bool mfused = allow_fused && low[w].regular && b->meta[w].margin_flag == 0 && low[w].nmpitems > 0;
-        b->meta[w].fused = fused ? 1 : 0; b->meta[w].mfused = mfused ? 1 : 0;
-        if (fused) { low[w].nitems_s = 0; low[w].nlist_s = 0; low[w].nph_s = 0; b->meta[w].nitems = 0; b->meta[w].nphases = 0; if (b->meta[w].has_common) n_fused_wide++; else n_fused_compact++; }
-        else { low[w].npitems = 0; low[w].nxrec = 0; n_unfused++; }
-        if (!fused || b->meta[w].has_common) { low[w].nrun = 0; low[w].nrtile = 0; }
-        if (mfused) { low[w].nitems_m = 0; low[w].nlist_m = 0; low[w].nph_m = 0; b->meta[w].nmitems = 0; b->meta[w].nmphases = 0; n_mfused++; }
-        else { low[w].nmpitems = 0; low[w].nmxrec = 0; if (b->meta[w].margin_flag == 0) n_munfused++; }
-        if (!(fused && b->meta[w].has_common) && !mfused) low[w].nlmb = 0;
+    for (const WinLow &lo : low) {
+        bd.n_unfused += lo.solve == SOLVE_UNFUSED; bd.n_fused_compact += lo.solve == SOLVE_COMPACT; bd.n_fused_wide += lo.solve == SOLVE_WIDE;
+        bd.n_munfused += lo.marg == MARG_UNFUSED; bd.n_mfused += lo.marg == MARG_WIDE;
     }
     // host runs, longest first (a counting sort by tile count): every window's long run (its frame-0 run, on the bench's windows) starts in the first
     // waves instead of forming the tail
     size_t nrun = 0, nrtile = 0;
     {
         int maxt = 0;
-        for (int w = 0; w < B; w++) for (int f = 0; f < NFR; f++) maxt = std::max(maxt, low[w].nrun ? low[w].run_nt[f] : 0);
+        for (int w = 0; w < B; w++) for (int f = 0; f < NFR; f++) maxt = std::max(maxt, low[w].run_nt[f]);
         std::vector<size_t> start((size_t)maxt + 2, 0);
-        for (int w = 0; w < B; w++) if (low[w].nrun) for (int f = 0; f < NFR; f++) if (low[w].run_nt[f]) start[maxt - low[w].run_nt[f] + 1]++;
+        for (int w = 0; w < B; w++) for (int f = 0; f < NFR; f++) if (low[w].run_nt[f]) start[maxt - low[w].run_nt[f] + 1]++;
         for (int t = 1; t <= maxt + 1; t++) start[t] += start[t - 1];
         for (int w = 0; w < B; w++) {
             WinLow &lo = low[w];
             lo.rtile_off = (int)nrtile; nrtile += lo.nrtile; nrun += lo.nrun;
-            if (lo.nrun) for (int f = 0; f < NFR; f++) if (lo.run_nt[f]) lo.run_slot[f] = (int)start[maxt - lo.run_nt[f]]++;
+            for (int f = 0; f < NFR; f++) if (lo.run_nt[f]) lo.run_slot[f] = (int)start[maxt - lo.run_nt[f]]++;
         }
     }
     // ---- phase 2: offsets
@@ -678,15 +671,15 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
         m.vis_off = (int)nvis; nvis += p.num_vis; m.lm_off = (int)nlm; nlm += p.num_landmarks;
         low[w].obsi_off = (int)nobsi; nobsi += lo.nobs_i;
         m.imu_off = (int)nimu; nimu += p.num_imu; m.wheel_off = (int)nwheel; nwheel += p.num_wheel; m.plane_off = (int)nplane; nplane += p.num_plane;
-        m.item_off = (int)nit_s; nit_s += lo.nitems_s; m.list_off = (int)nlist; nlist += lo.nlist_s;
+        m.item_off = (int)nit_s; nit_s += m.nitems; m.list_off = (int)nlist; nlist += lo.nlist_s;
         m.prior_idx = lo.has_prior ? (int)npri++ : -1;
-        m.lmb_off = (int)nlmb; m.nlmb = lo.nlmb; nlmb += lo.nlmb; m.pitem_off = (int)npit; m.npitems = lo.npitems; npit += lo.npitems; m.xrec_off = (int)nxr; m.nxrec = lo.nxrec; nxr += (size_t)lo.nxrec * (m.has_common ? (int)XL<true>::REC : (int)XL<false>::REC);
-        m.mpitem_off = (int)nmpit; m.nmpitems = lo.nmpitems; nmpit += lo.nmpitems; m.mxrec_off = (int)nmxr; m.nmxrec = lo.nmxrec; nmxr += (size_t)lo.nmxrec * XL<true>::REC;
+        m.lmb_off = (int)nlmb; nlmb += m.nlmb; m.pitem_off = (int)npit; npit += m.npitems; m.xrec_off = (int)nxr; nxr += (size_t)m.nxrec * XL<true>::REC;      // (only wide solver windows store records)
+        m.mpitem_off = (int)nmpit; nmpit += m.nmpitems; m.mxrec_off = (int)nmxr; nmxr += (size_t)m.nmxrec * XL<true>::REC;
         b->prior_n[w] = lo.prior_n_out; if (m.margin_flag >= 0) b->any_marg = true;
         b->prior_nmax = std::max(b->prior_nmax, lo.prior_n_out);
         b->algorithmic_bytes += window_algorithmic_bytes(p, opt->max_num_iterations);
     }
-    for (int w = 0; w < B; w++) { WinMeta &m = b->meta[w]; const WinLow &lo = low[w]; m.mitem_off = (int)nit_m; nit_m += lo.nitems_m; m.mlist_off = (int)nlist; nlist += lo.nlist_m; }
+    for (int w = 0; w < B; w++) { WinMeta &m = b->meta[w]; m.mitem_off = (int)nit_m; nit_m += m.nmitems; m.mlist_off = (int)nlist; nlist += low[w].nlist_m; }
     if (nxr > 0x7fffffff || nmxr > 0x7fffffff || nstate > 0x7fffffff || nvis * 12 > 0x7fffffffull * 4 || nlist > 0x7fffffff) { batch_free(ctx, b); return fail(ctx, VIWB_ERR_INVALID, "batch too large"); }
     std::vector<PriorDev> priors(npri);
     for (int w = 0; w < B; w++) if (b->meta[w].prior_idx >= 0) {
@@ -701,7 +694,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     bd.nvis_total = (int)nvis; bd.nlm_total = (int)nlm; bd.nimu_total = (int)nimu; bd.nwheel_total = (int)nwheel; bd.nplane_total = (int)nplane; bd.nprior = (int)npri;
     bd.nitems_solve = (int)nit_s; bd.nitems_marg = (int)nit_m;
     bd.rec_stride_solve = VREC_COMPACT;
-    bd.n_unfused = n_unfused; bd.nlmb_total = (int)nlmb; bd.npitems_total = (int)npit; bd.nmpitems_total = (int)nmpit; bd.nrun_total = (int)nrun;
+    bd.nlmb_total = (int)nlmb; bd.npitems_total = (int)npit; bd.nmpitems_total = (int)nmpit; bd.nrun_total = (int)nrun;
     bd.pitems_max = 1; for (int w = 0; w < B; w++) bd.pitems_max = std::max(bd.pitems_max, std::max(b->meta[w].npitems, b->meta[w].nmpitems));
     {   // pair_win keeps a window's chunk products in shared memory: possible when the largest window fits next to a second resident block
         size_t need_s = 0, need_m = 0;
@@ -711,32 +704,38 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
             if (mw.mfused) need_m = std::max(need_m, pair_win_smem_bytes(mw.nmpitems, (int)XL<true>::OUT));
         }
         const size_t cap = 110 * 1024;
-        bd.pwin_smem = (!g_no_pair_win && n_fused_compact == 0 && need_s > 0 && need_s <= cap) ? (int)need_s : 0;
+        bd.pwin_smem = (!g_no_pair_win && bd.n_fused_compact == 0 && need_s > 0 && need_s <= cap) ? (int)need_s : 0;
         bd.pwin_smem_marg = (!g_no_pair_win && need_m > 0 && need_m <= cap) ? (int)need_m : 0;
     }
-    bd.n_fused_wide = n_fused_wide; bd.n_fused_compact = n_fused_compact; bd.n_mfused = n_mfused; bd.n_munfused = n_munfused;
-    bd.pout_stride = n_fused_wide ? (int)XL<true>::OUT : (int)XL<false>::OUT;
+    bd.pout_stride = bd.n_fused_wide ? (int)XL<true>::OUT : (int)XL<false>::OUT;
     bd.marg_nmax = b->prior_nmax;
     bd.env_max = 1; for (int w = 0; w < B; w++) bd.env_max = std::max(bd.env_max, b->meta[w].esize);
     for (int w = 0; w < B; w++) if (b->meta[w].has_common) bd.rec_stride_solve = VREC;
     b->total_state = nstate;
-    // ---- placement (inputs first, then work arrays)
-    struct Ent { void **field; size_t bytes; bool input; size_t off; };
+    // ---- the slab: every array once -- its device field, its element count, and for an input its view in the staging slab (HostArrays).
+    // Inputs come first and are uploaded as one block; a work array is never empty.
+    struct Ent { void **dev, **host; size_t bytes, off; };
     std::vector<Ent> ents;
-    auto IN = [&](auto **field, size_t count) { ents.push_back({(void **)field, count * sizeof(**field), true, 0}); };
-    auto WK = [&](auto **field, size_t count) { ents.push_back({(void **)field, (count ? count : 1) * sizeof(**field), false, 0}); };
-    IN(&bd.meta, B); IN(&bd.prior, npri); IN(&bd.vis_code, nvis); IN(&bd.vis_lm, nvis); IN(&bd.vis_oi, nvis);
-    IN(&bd.obs_i, nobsi * 6); IN(&bd.obs_j, nvis * 6); IN(&bd.lm_win, nlm); IN(&bd.lm_fptr, nlm + 1); IN(&bd.items, nit_s + nit_m); IN(&bd.asm_list, nlist);
-    IN(&bd.imu_fi, nimu); IN(&bd.imu_fj, nimu); IN(&bd.imu_win, nimu); IN(&bd.wheel_fi, nwheel); IN(&bd.wheel_fj, nwheel); IN(&bd.wheel_win, nwheel);
-    IN(&bd.plane_f, nplane); IN(&bd.plane_win, nplane); IN(&bd.imu_data, nimu * 287); IN(&bd.wheel_data, nwheel * 78);
-    IN(&bd.prior_J, npJ); IN(&bd.prior_r, npr); IN(&bd.prior_x0, npri * SFIX); IN(&bd.x_init, nstate); IN(&b->work_init_dev, B);
-    IN(&bd.vis_pos, n_fused_wide ? nvis : 0); IN(&bd.lmb_desc, nlmb); IN(&bd.pitems, npit);
-    IN(&bd.mvis_pos, nmpit ? nvis : 0); IN(&bd.mpitems, nmpit);
-    IN(&bd.run_desc, nrun); IN(&bd.run_tile, nrtile); IN(&bd.run_f, nrun ? nvis : 0); IN(&bd.run_lm, nrun ? 2 * nlm : 0);
+    HostArrays h; memset(&h, 0, sizeof h);
+    auto IN = [&](auto **dev, auto *&host, size_t count) {
+        static_assert(std::is_same<std::remove_const_t<std::remove_reference_t<decltype(**dev)>>, std::remove_reference_t<decltype(*host)>>::value, "host view of another type");
+        ents.push_back({(void **)dev, (void **)&host, count * sizeof(*host), 0});
+    };
+    auto WK = [&](auto **dev, size_t count) { ents.push_back({(void **)dev, nullptr, (count ? count : 1) * sizeof(**dev), 0}); };
+    IN(&bd.meta, h.meta, B); IN(&bd.prior, h.prior, npri); IN(&bd.vis_code, h.vis_code, nvis); IN(&bd.vis_lm, h.vis_lm, nvis); IN(&bd.vis_oi, h.vis_oi, nvis);
+    IN(&bd.obs_i, h.obs_i, nobsi * 6); IN(&bd.obs_j, h.obs_j, nvis * 6); IN(&bd.lm_win, h.lm_win, nlm); IN(&bd.lm_fptr, h.lm_fptr, nlm + 1);
+    IN(&bd.items, h.items, nit_s + nit_m); IN(&bd.asm_list, h.asm_list, nlist);
+    IN(&bd.imu_fi, h.imu_fi, nimu); IN(&bd.imu_fj, h.imu_fj, nimu); IN(&bd.imu_win, h.imu_win, nimu); IN(&bd.wheel_fi, h.wheel_fi, nwheel); IN(&bd.wheel_fj, h.wheel_fj, nwheel); IN(&bd.wheel_win, h.wheel_win, nwheel);
+    IN(&bd.plane_f, h.plane_f, nplane); IN(&bd.plane_win, h.plane_win, nplane); IN(&bd.imu_data, h.imu_data, nimu * 287); IN(&bd.wheel_data, h.wheel_data, nwheel * 78);
+    IN(&bd.prior_J, h.prior_J, npJ); IN(&bd.prior_r, h.prior_r, npr); IN(&bd.prior_x0, h.prior_x0, npri * SFIX); IN(&bd.x_init, h.x_init, nstate); IN(&b->work_init_dev, h.work, B);
+    IN(&bd.vis_pos, h.vis_pos, bd.n_fused_wide ? nvis : 0); IN(&bd.lmb_desc, h.lmb_desc, nlmb); IN(&bd.pitems, h.pitems, npit);
+    IN(&bd.mvis_pos, h.mvis_pos, nmpit ? nvis : 0); IN(&bd.mpitems, h.mpitems, nmpit);
+    IN(&bd.run_desc, h.run_desc, nrun); IN(&bd.run_tile, h.run_tile, nrtile); IN(&bd.run_f, h.run_f, nrun ? nvis : 0); IN(&bd.run_lm, h.run_lm, nrun ? 2 * nlm : 0);
     const size_t nvec = (size_t)B * TFIX + nlm;
+    const bool any_unfused = bd.n_unfused || bd.n_munfused;      // lin_vis' per-factor records and costs
     WK(&bd.work, B); WK(&bd.x_cur, nstate); WK(&bd.x_cand, nstate); WK(&bd.x_before, nstate);
     WK(&bd.vis_type, nvis); WK(&bd.vis_fi, nvis); WK(&bd.vis_fj, nvis); WK(&bd.vis_win, nvis); WK(&bd.vis_dup, nvis); WK(&bd.vis_obs, nvis * 12);
-    WK(&bd.vis_rec, nvis * VREC); WK(&bd.vis_cost, nvis);
+    WK(&bd.vis_rec, any_unfused ? nvis * VREC : 0); WK(&bd.vis_cost, any_unfused ? nvis : 0);
     WK(&bd.xrec, std::max(nxr, nmxr)); WK(&bd.pair_out, npit * (size_t)bd.pout_stride); WK(&bd.mpair_out, nmpit * (size_t)XL<true>::OUT); WK(&bd.pair_red, (npit || nmpit) ? (size_t)B * PAIR_RED : 0);
     WK(&bd.lm_a, nlm); WK(&bd.lm_g, nlm); WK(&bd.lm_gamma, nlm); WK(&bd.lm_scale, nlm); WK(&bd.lm_cost, nlm); WK(&bd.lm_W, nlm * VSUB); WK(&bd.lm_outlier, nlm);
     WK(&bd.imu_S, nimu * 225); WK(&bd.wheel_S, nwheel * 36); WK(&bd.imu_rec, nimu * IMU_REC); WK(&bd.wheel_rec, nwheel * WHEEL_REC); WK(&bd.plane_rec, nplane * PLANE_REC);
@@ -749,9 +748,9 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     WK(&bd.marg_J, mB * mJ); WK(&bd.marg_r, mB * MAXPRI); WK(&bd.marg_x0, mB * SFIX);
     WK(&bd.marg_hdr, mB * (3 + 2 * NB)); WK(&bd.marg_de, mB * 2 * MAXPRI); WK(&bd.marg_rot, mB * 2 * marg_rot_cap(b->prior_nmax)); WK(&bd.marg_sweep, mB * (2 * marg_sweep_cap(b->prior_nmax) + 2));
     size_t tot = 0;
-    for (auto &e : ents) if (e.input) { e.off = tot; tot += align_up(e.bytes); }
+    for (auto &e : ents) if (e.host) { e.off = tot; tot += align_up(e.bytes); }
     const size_t in_bytes = tot;
-    for (auto &e : ents) if (!e.input) { e.off = tot; tot += align_up(e.bytes); }
+    for (auto &e : ents) if (!e.host) { e.off = tot; tot += align_up(e.bytes); }
     b->out_bytes = align_up(nstate * 8) + align_up(sizeof(WinWork) * B) + align_up((size_t)B * (3 + 2 * NB) * 4) + align_up((size_t)B * MAXPRI * 8) +
                    align_up((size_t)B * SFIX * 8) + align_up((size_t)B * b->prior_nmax * b->prior_nmax * 8);
     b->out_off = align_up(in_bytes);
@@ -762,17 +761,8 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     if (ar->host_cap < host_need) { if (ar->host) host_free(ar->host); ar->host = nullptr; ar->host_cap = 0; void *hm = nullptr; int e = host_alloc(&hm, host_need + host_need / 8); if (e) { batch_free(ctx, b); return fail(ctx, VIWB_ERR_CUDA, "pinned staging slab"); } ar->host = (char *)hm; ar->host_cap = host_need + host_need / 8; }
     if (b->arena_cached) b->arena = *ar;     // a view; ownership stays with the context
     const double t_alloc = now_ms();
-    // host views of the input arrays inside the staging slab
-    HostArrays h; memset(&h, 0, sizeof h);
-    { size_t k = 0; char *hb = ar->host;
-      auto HP = [&](auto *&dst) { dst = (typename std::remove_reference<decltype(dst)>::type)(hb + ents[k].off); k++; };
-      HP(h.meta); HP(h.prior); HP(h.vis_code); HP(h.vis_lm); HP(h.vis_oi); HP(h.obs_i); HP(h.obs_j); HP(h.lm_win); HP(h.lm_fptr); HP(h.items); HP(h.asm_list);
-      HP(h.imu_fi); HP(h.imu_fj); HP(h.imu_win); HP(h.wheel_fi); HP(h.wheel_fj); HP(h.wheel_win); HP(h.plane_f); HP(h.plane_win); HP(h.imu_data); HP(h.wheel_data);
-      HP(h.prior_J); HP(h.prior_r); HP(h.prior_x0); HP(h.x_init); HP(h.work);
-      HP(h.vis_pos); HP(h.lmb_desc); HP(h.pitems); HP(h.mvis_pos); HP(h.mpitems);
-      HP(h.run_desc); HP(h.run_tile); HP(h.run_f); HP(h.run_lm); }
+    for (auto &e : ents) { *e.dev = ar->dev + e.off; if (e.host) *e.host = ar->host + e.off; }
     h.nitems_solve_total = (int)nit_s;
-    for (auto &e : ents) *e.field = ar->dev + e.off;
     if (npri) memcpy(h.prior, priors.data(), sizeof(PriorDev) * npri);
     h.lm_fptr[nlm] = (int)nvis;
     // ---- phase 3 (parallel): fill
@@ -830,46 +820,38 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
     // cost_only: the round after the last allowed iteration only decides accept / reject of the pending candidate (every window
     // still running is at max_num_iterations there, trust_region_minimizer.cc checks the iteration limit before the gradient),
     // so the partial sums and the Schur product of that linearisation would never be read
+    // one linearisation: visual kernels of the fused paths, then of the unfused windows, the small factors, (the accept / reject decision stops here),
+    // the fused paths' pair products, the unfused windows' gather sums, and the Schur product
     auto lin = [&](int mode, bool cost_only) {
         const bool solve = mode == MODE_SOLVE;
-        const bool old_path = solve ? bd.n_unfused > 0 : bd.n_munfused > 0;      // windows outside the fused path (irregular factor tables)
-        const int wpb2 = NT(128) / (NT(128) < 32 ? NT(128) : 32);
-        const int nfi = solve ? bd.npitems_total : bd.nmpitems_total;               // fused pair items of this mode
-        if (solve) {
-            const int vmode = cost_only ? (int)MODE_COST : mode;
-            if (bd.n_fused_compact > 0) { LAUNCH(lin_vis_lm, bd, bd.nrun_total, 1, NT(LMB_FACTORS), lin_vis_run_smem_doubles() * 8, vmode, st); ctx->launches++; }      // + the compact windows' pair chunks
-            if (bd.n_fused_wide > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, vmode, st); ctx->launches++; }
-        } else if (bd.n_mfused > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, mode, st); ctx->launches++; }
-        auto fused_asm = [&]() {
-            if (nfi <= 0) return;
-            const int pw = solve ? bd.pwin_smem : bd.pwin_smem_marg;
-            if (pw > 0) { LAUNCH(pair_win, bd, B, 1, NT(256), (size_t)pw, mode, st); ctx->launches++; return; }
-            if (!solve || bd.n_fused_wide > 0) { LAUNCH(asm_pairs_wide, bd, (nfi + wpb2 - 1) / wpb2, 1, NT(128), 0, mode, st); ctx->launches++; }
-            LAUNCH(pair_reduce, bd, B, 1, NT(PAIR_RED_NT), (size_t)bd.pitems_max * sizeof(int), mode, st); ctx->launches++;
-        };
-        if (!old_path) {
-            LAUNCH(lin_small, bd, B, 1, nt_small, sm_small, mode, st); ctx->launches++;
-            if (cost_only) return;
-            fused_asm();
-            if (g_syrk_dfma) LAUNCH(syrk, bd, B, 1, nt_syrk, syrk_smem_doubles() * 8, mode, st);
-            else LAUNCH(syrk_mma, bd, B, 1, NT(SYRK_NT), syrk_mma_smem_doubles() * 8, mode, st);
-            ctx->launches++;
-            return;
+        const bool unfused = solve ? bd.n_unfused > 0 : bd.n_munfused > 0;      // windows outside the fused path (irregular factor tables)
+        const int rs = solve ? bd.rec_stride_solve : (int)VREC;      // the unfused records (VREC: they and the items carry the common columns)
+        const int vmode = cost_only ? (int)MODE_COST : mode;
+        if (solve && bd.n_fused_compact > 0) { LAUNCH(lin_vis_lm, bd, bd.nrun_total, 1, NT(LMB_FACTORS), lin_vis_run_smem_doubles() * 8, vmode, st); ctx->launches++; }      // + the compact windows' pair chunks
+        if (solve ? bd.n_fused_wide > 0 : bd.n_mfused > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, vmode, st); ctx->launches++; }
+        if (unfused) {
+            LAUNCH(lin_vis, bd, g_vis, 1, nt_vis, lin_vis_smem_doubles(nt_vis, rs) * 8, mode, st);
+            if (rs == VREC) LAUNCH(lm_reduce_wide, bd, g_lm, 1, nt_lm, 0, mode, st);
+            else LAUNCH(lm_reduce, bd, g_lm, 1, nt_lm, 0, mode, st);
+            ctx->launches += (g_vis > 0) + (g_lm > 0);
         }
-        LAUNCH(lin_vis, bd, g_vis, 1, nt_vis, lin_vis_smem_doubles(nt_vis, mode == MODE_SOLVE ? bd.rec_stride_solve : (int)VREC) * 8, mode, st);
-        if ((mode == MODE_SOLVE ? bd.rec_stride_solve : (int)VREC) == VREC) LAUNCH(lm_reduce_wide, bd, g_lm, 1, nt_lm, 0, mode, st);
-        else LAUNCH(lm_reduce, bd, g_lm, 1, nt_lm, 0, mode, st);
-        LAUNCH(lin_small, bd, B, 1, nt_small, sm_small, mode, st);
-        ctx->launches += (g_vis > 0) + (g_lm > 0) + 1;
+        LAUNCH(lin_small, bd, B, 1, nt_small, sm_small, mode, st); ctx->launches++;
         if (cost_only) return;
-        const int ni = mode == MODE_SOLVE ? bd.nitems_solve : bd.nitems_marg, wpb = nt_asm / (nt_asm < 32 ? nt_asm : 32);
-        const bool wide = (mode == MODE_SOLVE ? bd.rec_stride_solve : (int)VREC) == VREC;     // items carry the common columns
-        fused_asm();
-        if (wide) LAUNCH(asm_items_split, bd, (ni * ASM_SPLIT + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
-        else LAUNCH(asm_items, bd, (ni + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
+        const int nfi = solve ? bd.npitems_total : bd.nmpitems_total, pw = solve ? bd.pwin_smem : bd.pwin_smem_marg, wpb = nt_asm / (nt_asm < 32 ? nt_asm : 32);
+        if (nfi > 0 && pw > 0) { LAUNCH(pair_win, bd, B, 1, NT(256), (size_t)pw, mode, st); ctx->launches++; }
+        else if (nfi > 0) {
+            if (!solve || bd.n_fused_wide > 0) { LAUNCH(asm_pairs_wide, bd, (nfi + wpb - 1) / wpb, 1, NT(128), 0, mode, st); ctx->launches++; }
+            LAUNCH(pair_reduce, bd, B, 1, NT(PAIR_RED_NT), (size_t)bd.pitems_max * sizeof(int), mode, st); ctx->launches++;
+        }
+        if (unfused) {
+            const int ni = solve ? bd.nitems_solve : bd.nitems_marg;
+            if (rs == VREC) LAUNCH(asm_items_split, bd, (ni * ASM_SPLIT + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
+            else LAUNCH(asm_items, bd, (ni + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
+            ctx->launches += ni > 0;
+        }
         if (g_syrk_dfma) LAUNCH(syrk, bd, B, 1, nt_syrk, syrk_smem_doubles() * 8, mode, st);
         else LAUNCH(syrk_mma, bd, B, 1, NT(SYRK_NT), syrk_mma_smem_doubles() * 8, mode, st);
-        ctx->launches += (ni > 0) + 1;
+        ctx->launches++;
     };
     if (what & (RUN_SOLVE | RUN_MARG | RUN_LIN_ONLY)) {
         const int ns = bd.nimu_total + bd.nwheel_total, nt_s = NT(128);
