@@ -192,7 +192,7 @@ VIWB_D void syrk_block(const BatchDev &bd, int bx, int by, int tid, int nt, doub
         async_commit();
         for (int k = tid; k < kc; k += nt) {
             double g = gam[k0 + k];
-            if (mode == MODE_MARG) g = g > 0.0 ? 1.0 / g : 0.0;
+            if (mode == MODE_MARG) g = marg_pivot_weight(g);
             gkb[p][k] = g; ggb[p][k] = g * gl[k0 + k];
         }
     };

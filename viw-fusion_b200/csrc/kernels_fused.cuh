@@ -524,7 +524,7 @@ VIWB_D void pair_win_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
 
 // ------------------------------------------------------------------------------------------------ syrk_mma
 // T = sum_k g_k w_k w_k^T (80 x 80, both triangles written, exactly symmetric), tvec = sum_k g_k gl_k w_k.
-// solver: g_k = gamma_k; marginalisation: g_k = 1 / a_k for the landmarks hosted in frame 0 (gamma holds a_k, 0 = skip).
+// solver: g_k = gamma_k; marginalisation: g_k = 1 / a_k for the landmarks hosted in frame 0 (gamma holds a_k, 0 = skip; marg_pivot_weight).
 // One [80 x K] x [K x 81] product (column 80 of the right operand = gl): 10 x 11 tiles of 8 x 8, of which the 55 upper-triangular ones
 // and the 10 of the tvec column are computed: five warps, warp v owns tile rows v and 9 - v (13 tiles each).  Chunks of 32 landmarks stream
 // through two shared-memory buffers (cp.async); the row stride 88 makes every operand fetch two conflict-free wavefronts.
@@ -543,7 +543,7 @@ VIWB_D void syrk_mma_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
     for (int i = 0; i < VSUB; i++) { for (int j = 0; j < VSUB; j++) T[i * VSUB + j] = 0.0; tv[i] = 0.0; }
     for (int k = 0; k < m.nlm; k++) {
         double g = gam[k];
-        if (mode == MODE_MARG) g = g > 0.0 ? 1.0 / g : 0.0;
+        if (mode == MODE_MARG) g = marg_pivot_weight(g);
         if (g == 0.0) continue;                           // a landmark that takes no part: its row of W is not even read (it may never have been written)
         const double *r = W + (size_t)k * VSUB;
         for (int i = 0; i < VSUB; i++) { const double a = g * r[i]; for (int j = i; j < VSUB; j++) T[i * VSUB + j] += a * r[j]; tv[i] += a * gl[k]; }
@@ -570,7 +570,7 @@ VIWB_D void syrk_mma_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
         async_commit();
         for (int r = tid; r < SYRK_KC; r += nt) {
             double g = 0.0, gg = 0.0;
-            if (r < kc) { g = gam[k0 + r]; if (mode == MODE_MARG) g = g > 0.0 ? 1.0 / g : 0.0; gg = gl[k0 + r]; }
+            if (r < kc) { g = gam[k0 + r]; if (mode == MODE_MARG) g = marg_pivot_weight(g); gg = gl[k0 + r]; }
             gkb[p][r] = g;
             Wb[p][r * SYRK_LD + VSUB] = gg;                   // column 80 of the right operand
             if (r >= kc) for (int q = 0; q < VSUB; q++) Wb[p][r * SYRK_LD + q] = 0.0;      // rows past the end of the window: zeros, not stale bytes

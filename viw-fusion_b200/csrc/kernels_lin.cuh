@@ -22,6 +22,11 @@ VIWB_HD int blk_moff(int b) { int t = blk_toff(b); return b > BLK_PR ? t + 1 : t
 // MARGIN_SECOND_NEW marginalises the prior only (estimator.cpp:1819-1842); margin_flag < 0: nothing to marginalise
 VIWB_HD bool marg_prior_only(const WinMeta &m, int mode) { return mode == MODE_MARG && m.margin_flag == 1; }
 VIWB_HD bool marg_skip(const WinMeta &m, int mode) { return mode == MODE_MARG && m.margin_flag < 0; }
+// Weight 1 / a of a dropped landmark's pivot a in the Schur sum T0 = sum w w^T / a.  The reference inverts the whole landmark block through its
+// eigenvalues and discards every eigenvalue <= 1e-8 (marginalization_factor.cpp:282-287); a pivot under that cut is discarded here the same way.
+// Such a pivot (a landmark seen only from its host's camera centre: no parallax) is rounding noise and so is its coupling w: its eigenvector is
+// the landmark's own axis to O(|w|^2), so dropping it equals the eigen-cut, while dividing by it would inject w w^T / a in a direction set by rounding.
+VIWB_HD double marg_pivot_weight(double a) { return a > 1e-8 ? 1.0 / a : 0.0; }
 
 VIWB_HD int rec_stride(const BatchDev &bd, int mode) { return mode == MODE_SOLVE ? bd.rec_stride_solve : VREC; }
 

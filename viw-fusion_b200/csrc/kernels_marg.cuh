@@ -46,96 +46,14 @@ VIWB_D void reanchor_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
     for (int k = 0; k < m.nlm; k++) st[SFIX + k] = 1.0 / (1.0 / st[SFIX + k]);   // setDepth(1/x), getDepthVector(1/depth)
 }
 
-// Symmetric eigen-decomposition in shared memory: Householder tridiagonalisation + implicit QL with eigenvector
-// accumulation (the EISPACK tred2 / tql2 pair, the algorithm family Eigen::SelfAdjointEigenSolver uses), with the
-// O(n^2)-per-step inner loops spread over the block and the O(n) scalar recurrences kept on thread 0.
-// V (n x n, leading dimension ld): in = symmetric matrix (lower triangle read), out = eigenvectors in columns.
-// d (n): eigenvalues (unsorted).  e (n), cs (2n), sc (8): scratch.
-VIWB_D double blk_reduce_small(double v, int tid, int nt, double *red) {     // sum over the block via a short tree
-    return block_sum(v, tid, nt, red);
-}
-// tri_only: stop after tred2 + the accumulation of the Householder transformations: V = Q, d = diagonal, e[0..n-2] = sub-diagonal, e[n-1] = 0
-VIWB_D void sym_eig_block(double *V, double *d, double *e, double *cs, double *sc, double *red, int n, int ld, int tid, int nt, bool tri_only = false) {
+// The implicit QL iteration (EISPACK tql2) with eigenvector accumulation, in shared memory: the second half of the eigen-decomposition that stands
+// in for Eigen::SelfAdjointEigenSolver, after tridiag_block.  The O(n) scalar recurrence runs on thread 0, the rotation of V's rows is spread over
+// the block.  In: V = Q of the tridiagonalisation (n x n, leading dimension ld), d (n) its diagonal, e (n) its sub-diagonal (e[n-1] = 0).
+// Out: V = eigenvectors in columns, d = eigenvalues (unsorted).  cs (2n), sc (8): scratch.
+VIWB_D void tql2_block(double *V, double *d, double *e, double *cs, double *sc, int n, int ld, int tid, int nt) {
 #define VV(i, j) V[(i) * ld + (j)]
-    // ---- tred2
-    for (int j = tid; j < n; j += nt) d[j] = VV(n - 1, j);
+    if (tid == 0) { sc[1] = 0.0 /* f */; sc[2] = 0.0 /* tst1 */; }
     VIWB_SYNC();
-    for (int i = n - 1; i > 0; i--) {
-        double part = 0.0;
-        for (int k = tid; k < i; k += nt) part += fabs(d[k]);
-        const double scale = blk_reduce_small(part, tid, nt, red);
-        if (scale == 0.0) {
-            if (tid == 0) e[i] = d[i - 1];
-            VIWB_SYNC();
-            for (int j = tid; j < i; j += nt) { d[j] = VV(i - 1, j); VV(i, j) = 0.0; VV(j, i) = 0.0; }
-            VIWB_SYNC();
-            if (tid == 0) d[i] = 0.0;
-            VIWB_SYNC();
-            continue;
-        }
-        part = 0.0;
-        for (int k = tid; k < i; k += nt) { const double t = d[k] / scale; d[k] = t; part += t * t; }
-        double h = blk_reduce_small(part, tid, nt, red);
-        if (tid == 0) {
-            const double f = d[i - 1];
-            double g = sqrt(h); if (f > 0) g = -g;
-            e[i] = scale * g; h = h - f * g; d[i - 1] = f - g; sc[0] = h;
-        }
-        VIWB_SYNC();
-        h = sc[0];
-        // e[j] = (A d)[j] over the leading i x i block (lower triangle storage); column i keeps the Householder vector
-        for (int j = tid; j < i; j += nt) {
-            double g = 0.0;
-            for (int k = 0; k <= j; k++) g += VV(j, k) * d[k];
-            for (int k = j + 1; k < i; k++) g += VV(k, j) * d[k];
-            cs[j] = g / h;            // e[j] / h, kept in cs until the reduction below is done
-            VV(j, i) = d[j];
-        }
-        VIWB_SYNC();
-        part = 0.0;
-        for (int j = tid; j < i; j += nt) part += cs[j] * d[j];
-        const double f2 = blk_reduce_small(part, tid, nt, red);
-        const double hh = f2 / (h + h);
-        for (int j = tid; j < i; j += nt) e[j] = cs[j] - hh * d[j];
-        VIWB_SYNC();
-        // rank-2 update of the lower triangle: V[k][j] -= d[j] e[k] + e[j] d[k],  j <= k < i
-        for (int k = tid; k < i; k += nt) { const double ek = e[k], dk = d[k]; for (int j = 0; j <= k; j++) VV(k, j) -= d[j] * ek + e[j] * dk; }
-        VIWB_SYNC();
-        for (int j = tid; j < i; j += nt) { cs[j] = VV(i - 1, j); VV(i, j) = 0.0; }
-        VIWB_SYNC();
-        for (int j = tid; j < i; j += nt) d[j] = cs[j];
-        if (tid == 0) d[i] = h;
-        VIWB_SYNC();
-    }
-    // ---- accumulate the transformations
-    for (int i = 0; i < n - 1; i++) {
-        if (tid == 0) { VV(n - 1, i) = VV(i, i); VV(i, i) = 1.0; }
-        VIWB_SYNC();
-        const double h = d[i + 1];
-        if (h != 0.0) {
-            for (int k = tid; k <= i; k += nt) d[k] = VV(k, i + 1) / h;
-            VIWB_SYNC();
-            for (int j = tid; j <= i; j += nt) {
-                double g = 0.0;
-                for (int k = 0; k <= i; k++) g += VV(k, i + 1) * VV(k, j);
-                for (int k = 0; k <= i; k++) VV(k, j) -= g * d[k];
-            }
-            VIWB_SYNC();
-        }
-        for (int k = tid; k <= i; k += nt) VV(k, i + 1) = 0.0;
-        VIWB_SYNC();
-    }
-    for (int j = tid; j < n; j += nt) { d[j] = VV(n - 1, j); VV(n - 1, j) = 0.0; }
-    VIWB_SYNC();
-    if (tid == 0) { VV(n - 1, n - 1) = 1.0; e[0] = 0.0; }
-    VIWB_SYNC();
-    // ---- tql2
-    for (int i = 1 + tid; i < n; i += nt) cs[i - 1] = e[i];
-    VIWB_SYNC();
-    for (int i = tid; i < n - 1; i += nt) e[i] = cs[i];
-    if (tid == 0) { e[n - 1] = 0.0; sc[1] = 0.0 /* f */; sc[2] = 0.0 /* tst1 */; }
-    VIWB_SYNC();
-    if (tri_only) return;
     const double eps = 2.220446049250313e-16;
     for (int l = 0; l < n; l++) {
         if (tid == 0) {
@@ -188,7 +106,7 @@ VIWB_D void sym_eig_block(double *V, double *d, double *e, double *cs, double *s
 #undef VV
 }
 
-// Householder tridiagonalisation + accumulation of the transformations (the tred2 half of sym_eig_block, same outputs: V = Q, d = diagonal,
+// Householder tridiagonalisation + accumulation of the transformations (EISPACK tred2, the first half before tql2_block; outputs: V = Q, d = diagonal,
 // e[0 .. n-2] = sub-diagonal, e[n-1] = 0), organised for the block instead of statement by statement.  The first version spent 59 % of its warp samples at
 // barriers (profiles/r02m_marg_tri_kernel.ncu.txt): 15 barriers per column with one thread per row walking up to n elements while the others waited.  Here
 //   * the scale, the squared norm and d[i-1] come out of ONE three-way reduction (h = sum d^2 / scale^2 instead of a second pass over d / scale),
@@ -517,8 +435,10 @@ VIWB_D void marg_prep_block(const BatchDev &bd, int bx, int by, int tid, int nt,
     }
 }
 
-// marg_eig: eigen-decomposition of the kept n x n block in shared memory (tred2 + tql2, the algorithm family of Eigen::SelfAdjointEigenSolver),
-// J_lin = sqrt(S) V^T, r_lin = sqrt(S^-1) V^T b (marginalization_factor.cpp:289-306), in place over A / b in HBM.
+// marg_eig: eigen-decomposition of the kept n x n block in shared memory (tridiag_block + tql2_block, the algorithm family of
+// Eigen::SelfAdjointEigenSolver), J_lin = sqrt(S) V^T, r_lin = sqrt(S^-1) V^T b (marginalization_factor.cpp:289-306), in place over A / b in HBM.
+// The three-kernel pipeline below runs the same statements in the same order (bit-identical priors in the emulation build; on the device the
+// two kernels' code differs at rounding level).
 // (A parallel cyclic Jacobi was measured here: 10 sweeps x 81 rounds of 2x2 block updates cost ten times the QL chain, profiles/r02c_*.)
 VIWB_HD size_t marg_eig_smem_doubles(int nt, int nmax) { (void)nt; const int c = marg_cap(nmax); return (size_t)c * (c | 1) + (size_t)6 * c + 96 + 16 + 8; }      // V | b | cs (2) | d | e | red (3 x 32: three-way block reductions) | bc
 VIWB_D void marg_eig_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
@@ -531,12 +451,13 @@ VIWB_D void marg_eig_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
     if (hdr[0] == 0) return;                                  // marg_prep gave up (kept dimension beyond the solver's capacity)
     const int n = hdr[1], cap = marg_cap(bd.marg_nmax), ld = n | 1;
     const double eps = 1e-8;
-    double *Vn = smem, *bn = Vn + (size_t)cap * (cap | 1), *cs = bn + cap, *ev = cs + 2 * cap, *ee = ev + cap, *red = ee + cap, *bc = red + 32;
+    double *Vn = smem, *bn = Vn + (size_t)cap * (cap | 1), *cs = bn + cap, *ev = cs + 2 * cap, *ee = ev + cap, *red = ee + cap, *bc = red + 96;
     double *Jout = bd.marg_J + (size_t)w * bd.marg_nmax * bd.marg_nmax, *rout = bd.marg_r + (size_t)w * MAXPRI;
     for (int e = tid; e < n * n; e += nt) { const int i = e / n, j = e - i * n; Vn[i * ld + j] = Jout[e]; }
     for (int i = tid; i < n; i += nt) bn[i] = rout[i];
     VIWB_SYNC();
-    sym_eig_block(Vn, ev, ee, cs, bc, red, n, ld, tid, nt);
+    tridiag_block(Vn, ev, ee, cs, red, n, ld, tid, nt);
+    tql2_block(Vn, ev, ee, cs, bc, n, ld, tid, nt);
     VIWB_SYNC();
     for (int e = tid; e < n * n; e += nt) {
         const int i = e / n, k = e - i * n;
@@ -559,7 +480,8 @@ VIWB_D void marg_eig_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
 //   marg_tri    block per window : A -> tridiagonal (d, e) + Q (tred2 and the accumulation), Q back to the window's marg_J slot
 //   marg_ql     warp per window  : lane 0 runs tql2 on (d, e) alone and LOGS the rotations (c, s) sweep by sweep; eigenvalues to d
 //   marg_apply  block per window : thread per row of Q applies the logged rotations (the eigenvector half of tql2), then J_lin, r_lin
-// Same arithmetic in the same order as sym_eig_block (the rotations are applied to each row in the order tql2 applies them).
+// Same arithmetic in the same order as marg_eig: the same tridiag_block, then tql2_block's scalar recurrence statement for statement on lane 0, and
+// its rotations applied to each row in the order tql2_block applies them.
 enum { MARG_ROT_PER_N2 = 3, MARG_SWEEP_PER_N = 12 };      // rotation-log capacity 3 n^2 (a typical run needs ~n^2), sweep-log capacity 12 n
 VIWB_HD size_t marg_rot_cap(int nmax) { const int c = marg_cap(nmax); return (size_t)MARG_ROT_PER_N2 * c * c; }
 VIWB_HD size_t marg_sweep_cap(int nmax) { return (size_t)MARG_SWEEP_PER_N * marg_cap(nmax); }
@@ -580,7 +502,7 @@ VIWB_D void marg_tri_block(const BatchDev &bd, int bx, int by, int tid, int nt, 
     for (int e = tid; e < n * n; e += nt) { const int i = e / n, j = e - i * n; Q[e] = Vn[i * ld + j]; }
     for (int i = tid; i < n; i += nt) { de[i] = ev[i]; de[MAXPRI + i] = ee[i]; }
 }
-// lane 0 of a warp: tql2 on the tridiagonal matrix (the scalar half of sym_eig_block's QL loop, statement for statement), rotations logged
+// lane 0 of a warp: tql2 on the tridiagonal matrix (the scalar half of tql2_block, statement for statement), rotations logged
 VIWB_D void marg_ql_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
     (void)by; (void)mode; (void)nt;
     const int w = bx;

@@ -917,7 +917,7 @@ static int batch_fetch(viwb_context *ctx, viwb_batch *b, double *const *states, 
         CK(dev_d2h(J, bd.marg_J, (size_t)B * nmax * nmax * 8, ctx->stream));     // window w's n x n block (row stride n) heads its nmax^2 slot
     }
     CK(dev_sync(ctx->stream));
-    std::atomic<int> rc_a(0);
+    std::atomic<int> marg_fail(0);
     parallel_for(B, [&](int w) {           // ~54 KB of prior per window: the unpack into the caller's buffers runs on the host pool
         if (states && states[w]) memcpy(states[w], x + b->meta[w].state_off, sizeof(double) * b->state_sizes[w]);
         if (summaries) {
@@ -938,7 +938,7 @@ static int batch_fetch(viwb_context *ctx, viwb_batch *b, double *const *states, 
                 memcpy(out->r, r + (size_t)w * MAXPRI, sizeof(double) * n);
                 memcpy(out->x0, x0 + (size_t)w * SFIX, sizeof(double) * SFIX);
             }
-            if (work[w].marg_status < 0) rc_a = VIWB_ERR_NUMERIC;
+            if (work[w].marg_status < 0) marg_fail = work[w].marg_status;
         } else if (mode == 1) {
             const HostPrior &hp = b->in_prior[w];
             out->valid = 1; out->n = hp.n; out->num_blocks = hp.nb;
@@ -946,8 +946,10 @@ static int batch_fetch(viwb_context *ctx, viwb_batch *b, double *const *states, 
             memcpy(out->x0, hp.x0.data(), sizeof(double) * SFIX); memcpy(out->J, hp.J.data(), sizeof(double) * hp.n * hp.n); memcpy(out->r, hp.r.data(), sizeof(double) * hp.n);
         } else { out->valid = 0; out->n = 0; out->num_blocks = 0; }
     });
-    const int rc = rc_a;
-    if (rc) return fail(ctx, rc, "marginalisation: kept dimension exceeds the shared-memory eigen solver");
+    // marg_status: -1 from marg_prep (kept block larger than marg_cap), -2 from marg_ql (rotation or sweep log full)
+    if (marg_fail == -1) return fail(ctx, VIWB_ERR_NUMERIC, "marginalisation: kept dimension exceeds the shared-memory eigen solver");
+    if (marg_fail == -2) return fail(ctx, VIWB_ERR_NUMERIC, "marginalisation: the QL iteration filled its rotation log");
+    if (marg_fail) return fail(ctx, VIWB_ERR_NUMERIC, "marginalisation failed");
     return 0;
 }
 
