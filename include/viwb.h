@@ -273,6 +273,15 @@ int viwb_triangulate(viwb_context *ctx, const double *state, int n, const int32_
  * re-express depth in the new frame 0.  uv: [n][3] first-observation points; R row-major 3x3 (camera-to-world), P [3]. */
 int viwb_shift_depth(viwb_context *ctx, int n, const double *uv, const double *depth_in, const double *marg_R, const double *marg_P,
                      const double *new_R, const double *new_P, double init_depth, double *depth_out);
+/* Estimator::predictPtsInNextFrame (estimator.cpp:2080-2113): constant-velocity next pose nextT = curT * (prevT^-1 * curT) from frames
+ * frame_count-1 and frame_count of `state` (getPoseInWorldFrame, :2066-2078); for every feature with depth > 0, num_obs >= 2 and
+ * start_frame + num_obs - 1 == frame_count: pts_cam in the predicted left camera.  The feature list is the caller's
+ * FeatureManager::feature (every feature with a depth, also those optimization() leaves out), not the window's landmark table.
+ * pt0: [n][3] first observation (feature_per_frame[0].point), extrinsics of camera 0 from `state`.  pts_cam: [n][3]; valid[n] = 1
+ * where the reference inserts the id into predictPts (other rows of pts_cam are 0).  frame_count < 2: every valid[k] = 0 (:2083).
+ * prevT^-1 is formed as the rigid inverse [R^T | -R^T p]. */
+int viwb_predict_pts(viwb_context *ctx, const double *state, int frame_count, int n, const int32_t *start_frame,
+                     const int32_t *num_obs, const double *pt0, const double *depth, double *pts_cam, uint8_t *valid);
 
 /* Batch of B independent windows (one per sequence), host buffers in, host buffers out. */
 int viwb_optimization_batch(viwb_context *ctx, int batch, const viwb_problem *problems, double *const *states,
@@ -439,6 +448,22 @@ int viwb_tracker_track(viwb_tracker *t, double cur_time, const uint8_t *const *l
  * [streams] row counts.  Any pointer may be NULL.  Synchronises. */
 int viwb_tracker_download(viwb_tracker *t, int32_t *n_left, int32_t *ids, int32_t *track_cnt, float *feat, int32_t *n_right,
                           int32_t *ids_right, float *feat_right);
+/* The estimator's way back into the sessions, once per estimator tick (estimator.cpp:841-843, MULTIPLE_THREAD == 0), for every stream:
+ * FeatureTracker::removeOutliers(remove_ids) (feature_tracker.cpp:739-755: stable reduceVector of prev_pts, ids, track_cnt; the id ->
+ * undistorted point maps stay as they are) and then, for the streams with has_prediction[s] != 0, FeatureTracker::setPrediction
+ * (:715-736): for each remaining row, the prediction with the row's id projected by m_camera[0]->spaceToPlane (pinhole + radtan,
+ * PinholeCamera.cc:520-542) and rounded to float as cv::Point2f does, else the row's prev_pts.  The prediction stays in HBM and is
+ * consumed by the next viwb_tracker_track, which must then be called with predict_pts == NULL (VIWB_ERR_INVALID otherwise, and the
+ * session stays as it was); hasPrediction is cleared by that tick (:279).
+ * n_remove / n_pred: [streams] list lengths; remove_ids, pred_ids: the streams' lists back to back; pred_pts_cam: [sum n_pred][3]
+ * camera-frame points (viwb_predict_pts' output, compacted to its valid rows).  An id listed twice behaves as in the reference's
+ * std::set / std::map: removed once; of several predictions for one id the last one counts (predictPts[id] = pts_cam).  Either half
+ * may be absent (n_remove == NULL / n_pred == NULL); n_pred needs has_prediction.  A call without the prediction half while an
+ * earlier call's prediction is still pending is VIWB_ERR_INVALID (its rows would no longer line up), as are a call before the
+ * first tick, a negative length, and a non-zero length with a NULL list.  viwb_tracker_download still returns the last tick's
+ * rows afterwards.  Asynchronous on the context stream. */
+int viwb_tracker_feedback(viwb_tracker *t, const int32_t *n_remove, const int32_t *remove_ids, const int32_t *n_pred,
+                          const int32_t *pred_ids, const double *pred_pts_cam, const uint8_t *has_prediction);
 /* compulsory HBM bytes of one tick: the new images read once by the pyramid and once by the detector, pyramid levels written, rows out */
 double viwb_tracker_algorithmic_bytes(const viwb_tracker *t);
 

@@ -1,6 +1,7 @@
 // kernels_feat.cuh -- per-landmark geometry around the window solve (SURVEY 8 f-3):
 //   FeatureManager::triangulate / triangulatePoint   estimator/feature_manager.cpp:198-213, 309-380
 //   FeatureManager::removeBackShiftDepth             estimator/feature_manager.cpp:457-493
+//   Estimator::predictPtsInNextFrame                 estimator/estimator.cpp:2080-2113
 // One thread per feature; everything is a handful of 3x3 / 4x4 operations.
 #pragma once
 #include "vmath.cuh"
@@ -79,6 +80,30 @@ VIWB_D void shift_depth_item(const ShiftArgs &a, int k) {
     a.depth_out[k] = pts_j.z > 0 ? pts_j.z : a.init_depth;
 }
 
+// Estimator::predictPtsInNextFrame (estimator.cpp:2080-2113).  nextT = curT * (prevT^-1 * curT) with prevT^-1 taken as the rigid inverse
+// [R^T | -R^T p] instead of the reference's general Matrix4d inverse: the two agree to rounding for a rotation block, and the parity tests
+// hold the result to 1e-9 against the reference's compiled code.
+struct PredictArgs { int n, frame_count; const double *state; const int *start_frame, *num_obs; const double *pt0, *depth; double *pts_cam; unsigned char *valid; };
+VIWB_D void predict_pts_item(const PredictArgs &a, int k) {
+    if (k >= a.n) return;
+    const double *x = a.state;
+    const int fc = a.frame_count, first = a.start_frame[k], nobs = a.num_obs[k];
+    const double depth = a.depth[k];
+    const bool ok = fc >= 2 && depth > 0 && nobs >= 2 && first + nobs - 1 == fc;             // :2083, :2094, :2099
+    a.valid[k] = ok ? 1 : 0;
+    V3 pts_cam = v3(0.0, 0.0, 0.0);
+    if (ok) {
+        const M3 Rc = qR(ldq(x + 7 * fc + 3)), Rp = qR(ldq(x + 7 * (fc - 1) + 3)), ric = qR(ldq(x + 176 + 3));
+        const V3 Pc = ld3(x + 7 * fc), Pp = ld3(x + 7 * (fc - 1)), tic = ld3(x + 176);
+        const M3 nextR = Rc * (transpose(Rp) * Rc);
+        const V3 nextP = Rc * tmul(Rp, Pc - Pp) + Pc;
+        const V3 pts_j = ric * (depth * ld3(a.pt0 + 3 * k)) + tic;
+        const V3 pts_w = qR(ldq(x + 7 * first + 3)) * pts_j + ld3(x + 7 * first);
+        const V3 pts_local = tmul(nextR, pts_w - nextP);
+        pts_cam = tmul(ric, pts_local - tic);
+    }
+    st3(a.pts_cam + 3 * k, pts_cam);
+}
 
 // FeatureTracker::undistortedPts (featureTracker/feature_tracker.cpp:606-617) -> PinholeCamera::liftProjective with the recursive
 // distortion model, n = 8 (camera_models/src/camera_models/PinholeCamera.cc:450-517, distortion :646-662), results narrowed to
@@ -113,6 +138,7 @@ VIWB_D void undistort_item(const UndistArgs &a, int i) {
 __global__ void undistort_kernel(UndistArgs a) { undistort_item(a, blockIdx.x * blockDim.x + threadIdx.x); }
 __global__ void triangulate_kernel(TriArgs a) { triangulate_item(a, blockIdx.x * blockDim.x + threadIdx.x); }
 __global__ void shift_depth_kernel(ShiftArgs a) { shift_depth_item(a, blockIdx.x * blockDim.x + threadIdx.x); }
+__global__ void predict_pts_kernel(PredictArgs a) { predict_pts_item(a, blockIdx.x * blockDim.x + threadIdx.x); }
 #endif
 
 }  // namespace viwb

@@ -7,6 +7,7 @@
 //   the stereo half: ids_right = ids, reduceVector by the stereo status, right undistort / velocity  :254-268
 //   prev_* = cur_* (:296-300) and the featureFrame rows (:307-350)
 // hasPrediction (:122-137): forward flow seeded with predict_pts at maxLevel 1, repeated at maxLevel 3 when fewer than 10 succeed.
+// Between two ticks, the estimator's way back into the session (estimator.cpp:841-843): removeOutliers (:739-755) and setPrediction (:715-736).
 //
 // One block per camera stream (these are 150-point lists); `tid` / `nt` = thread index / count, the emulation build runs nt = 1.
 #pragma once
@@ -30,7 +31,7 @@ struct TrkArgs {                         // one camera stream; every array holds
     int *mapL_ids; float *mapL_un; int *mapL_n;      // prev_un_pts_map
     int *mapR_ids; float *mapR_un; int *mapR_n;      // prev_un_right_pts_map
     // --- prediction
-    const uint8_t *has_pred; int *pred_n, *redo_n;
+    uint8_t *has_pred; int *pred_n, *redo_n;
     // --- featureFrame rows: {x, y, u, v, vx, vy} (z = 1), left rows in cur_pts order, right rows in ids_right order
     int *out_n; int *out_ids, *out_cnt; float *out_feat;
     int *out_nr; int *out_ids_r; float *out_feat_r;
@@ -88,6 +89,72 @@ VIWB_D void trk_pred_check(const TrkArgs &a, int tid, int nt) {
         succ += tot;
     }
     if (tid == 0) *a.redo_n = succ < 10 ? n : 0;
+}
+
+// ---- between two ticks: FeatureTracker::removeOutliers then FeatureTracker::setPrediction, one warp per stream.
+// The id lists arrive sorted and free of duplicates (the host orders them as the reference's std::set / std::map do), stream f's slice is
+// [off[f], off[f + 1]).
+struct TrkFeedback { const int *rm_off, *rm_ids, *pr_off, *pr_ids; const double *pr_pts; const uint8_t *pr_flag; float *pred_pts; };
+
+VIWB_D int trk_find_id(const int *ids, int n, int id) {          // position of id in the ascending list, -1 when absent
+    int lo = 0, hi = n;
+    while (lo < hi) { const int mid = (lo + hi) >> 1; if (ids[mid] < id) lo = mid + 1; else hi = mid; }
+    return (lo < n && ids[lo] == id) ? lo : -1;
+}
+// PinholeCamera::spaceToPlane (PinholeCamera.cc:520-542, distortion :646-662) narrowed to cv::Point2f (feature_tracker.cpp:730).  Every
+// product and sum is rounded on its own (no fused multiply-add), so that the pixel is the float the reference's build (-ffp-contract=off
+// here, SSE2 there) hands to calcOpticalFlowPyrLK, bit for bit.
+#ifdef VIWB_HOST_EMU
+static inline double trk_mul(double a, double b) { return a * b; }
+static inline double trk_add(double a, double b) { return a + b; }
+#else
+VIWB_D double trk_mul(double a, double b) { return __dmul_rn(a, b); }
+VIWB_D double trk_add(double a, double b) { return __dadd_rn(a, b); }
+#endif
+VIWB_D void trk_space_to_plane(const TrkCam &c, const double *P, float &u, float &v) {
+    const double x = P[0] / P[2], y = P[1] / P[2];
+    double xd = x, yd = y;
+    if (!(c.k1 == 0.0 && c.k2 == 0.0 && c.p1 == 0.0 && c.p2 == 0.0)) {       // m_noDistortion
+        const double mx2 = trk_mul(x, x), my2 = trk_mul(y, y), mxy = trk_mul(x, y), rho2 = trk_add(mx2, my2);
+        const double rad = trk_add(trk_mul(c.k1, rho2), trk_mul(trk_mul(c.k2, rho2), rho2));
+        const double dx = trk_add(trk_add(trk_mul(x, rad), trk_mul(trk_mul(2.0, c.p1), mxy)), trk_mul(c.p2, trk_add(rho2, trk_mul(2.0, mx2))));
+        const double dy = trk_add(trk_add(trk_mul(y, rad), trk_mul(trk_mul(2.0, c.p2), mxy)), trk_mul(c.p1, trk_add(rho2, trk_mul(2.0, my2))));
+        xd = trk_add(x, dx); yd = trk_add(y, dy);
+    }
+    u = (float)trk_add(trk_mul(c.fx, xd), c.cx); v = (float)trk_add(trk_mul(c.fy, yd), c.cy);
+}
+VIWB_D void trk_feedback(const TrkArgs &a, const TrkRun &r, const TrkFeedback &fb, int f, int tid, int nt) {
+    const int n = *a.n_temporal;
+    int m = n;
+    if (fb.rm_off) {
+        // reduceVector(prev_pts / ids / track_cnt, status) in place: a row moves to a lower or equal index, so every thread of a group reads
+        // its row before any thread of the group writes
+        const int *rm = fb.rm_ids + fb.rm_off[f]; const int nrm = fb.rm_off[f + 1] - fb.rm_off[f];
+        m = 0;
+        for (int base = 0; base < n; base += nt) {
+            const int i = base + tid; int tot;
+            float u = 0.f, v = 0.f; int id = 0, cnt = 0;
+            if (i < n) { u = a.prev_pts[2 * i]; v = a.prev_pts[2 * i + 1]; id = a.ids[i]; cnt = a.track_cnt[i]; }
+            const bool keep = i < n && trk_find_id(rm, nrm, id) < 0;
+            const int j = m + trk_rank(keep, tid, tot);
+            VIWB_SYNCWARP();
+            if (keep) { a.prev_pts[2 * j] = u; a.prev_pts[2 * j + 1] = v; a.ids[j] = id; a.track_cnt[j] = cnt; }
+            m += tot;
+        }
+        VIWB_SYNCWARP();
+    }
+    const bool hp = fb.pr_off && fb.pr_flag[f] != 0;
+    if (hp) {
+        const int *pid = fb.pr_ids + fb.pr_off[f]; const int np = fb.pr_off[f + 1] - fb.pr_off[f];
+        float *out = fb.pred_pts + (size_t)f * r.maxn * 2;
+        for (int j = tid; j < m; j += nt) {
+            const int k = trk_find_id(pid, np, a.ids[j]);
+            float u = a.prev_pts[2 * j], v = a.prev_pts[2 * j + 1];                // no prediction for this id: predict_pts[i] = prev_pts[i]
+            if (k >= 0) trk_space_to_plane(r.cam[0], fb.pr_pts + 3 * ((size_t)fb.pr_off[f] + k), u, v);
+            out[2 * j] = u; out[2 * j + 1] = v;
+        }
+    }
+    if (tid == 0) { *a.n_temporal = m; *a.n_stereo = m; *a.has_pred = hp ? 1 : 0; }
 }
 
 // ---- stage 1, after the temporal flow: reduceVector by status and track_cnt++ straight into the detector's setMask input
@@ -168,6 +235,7 @@ __global__ void trk_pred_check_kernel(TrkRun r) { trk_pred_check(r.tasks[blockId
 __global__ void trk_advance_kernel(TrkRun r) { trk_advance(r.tasks[blockIdx.x], threadIdx.x, 32); }
 __global__ void trk_merge_kernel(TrkRun r) { trk_merge(r.tasks[blockIdx.x], r, threadIdx.x, blockDim.x); }
 __global__ void trk_stereo_kernel(TrkRun r) { trk_stereo(r.tasks[blockIdx.x], r, threadIdx.x, 32); }
+__global__ void trk_feedback_kernel(TrkRun r, TrkFeedback fb) { trk_feedback(r.tasks[blockIdx.x], r, fb, blockIdx.x, threadIdx.x, 32); }
 #endif
 
 }  // namespace viwb

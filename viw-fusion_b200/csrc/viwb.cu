@@ -1525,6 +1525,44 @@ extern "C" int viwb_shift_depth(viwb_context *ctx, int n, const double *uv, cons
     dev_free(d);
     return e ? fail(ctx, VIWB_ERR_CUDA, "shift_depth failed") : VIWB_OK;
 }
+// Estimator::predictPtsInNextFrame (estimator.cpp:2080-2113): thread per feature of the caller's FeatureManager::feature list
+extern "C" int viwb_predict_pts(viwb_context *ctx, const double *state, int frame_count, int n, const int32_t *start_frame, const int32_t *num_obs, const double *pt0,
+                                const double *depth, double *pts_cam, uint8_t *valid) {
+    if (!ctx || !state || n < 0 || !start_frame || !num_obs || !pt0 || !depth || !pts_cam || !valid) return VIWB_ERR_INVALID;
+    if (frame_count < 0 || frame_count > VIWB_WINDOW_SIZE) return fail(ctx, VIWB_ERR_INVALID, "predict_pts: frame_count out of the window");
+    for (int k = 0; k < n; k++) if (start_frame[k] < 0 || start_frame[k] > VIWB_WINDOW_SIZE || num_obs[k] < 0) return fail(ctx, VIWB_ERR_INVALID, "predict_pts: start_frame out of the window or negative num_obs");
+    if (n == 0) return VIWB_OK;
+    bind_device(ctx);
+    const size_t bytes = align_up(SFIX * 8) + 2 * align_up((size_t)n * 4) + 2 * align_up((size_t)n * 24) + align_up((size_t)n * 8) + align_up((size_t)n);
+    char *d = nullptr; CK(dev_malloc((void **)&d, bytes));
+    size_t o = 0;
+    double *d_x = (double *)(d + o); o += align_up(SFIX * 8);
+    int *d_sf = (int *)(d + o); o += align_up((size_t)n * 4);
+    int *d_no = (int *)(d + o); o += align_up((size_t)n * 4);
+    double *d_p0 = (double *)(d + o); o += align_up((size_t)n * 24);
+    double *d_out = (double *)(d + o); o += align_up((size_t)n * 24);
+    double *d_dep = (double *)(d + o); o += align_up((size_t)n * 8);
+    uint8_t *d_val = (uint8_t *)(d + o);
+    int e = dev_h2d(d_x, state, SFIX * 8, ctx->stream);
+    if (!e) e = dev_h2d(d_sf, start_frame, (size_t)n * 4, ctx->stream);
+    if (!e) e = dev_h2d(d_no, num_obs, (size_t)n * 4, ctx->stream);
+    if (!e) e = dev_h2d(d_p0, pt0, (size_t)n * 24, ctx->stream);
+    if (!e) e = dev_h2d(d_dep, depth, (size_t)n * 8, ctx->stream);
+    PredictArgs a; a.n = n; a.frame_count = frame_count; a.state = d_x; a.start_frame = d_sf; a.num_obs = d_no; a.pt0 = d_p0; a.depth = d_dep; a.pts_cam = d_out; a.valid = d_val;
+    if (!e) {
+#ifdef VIWB_HOST_EMU
+        for (int k = 0; k < n; k++) predict_pts_item(a, k);
+#else
+        g_prof.begin("predict_pts", ctx->stream); predict_pts_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
+#endif
+        ctx->launches++;
+        e = dev_d2h(pts_cam, d_out, (size_t)n * 24, ctx->stream);
+        if (!e) e = dev_d2h(valid, d_val, (size_t)n, ctx->stream);
+    }
+    if (!e) e = dev_sync(ctx->stream);
+    dev_free(d);
+    return e ? fail(ctx, VIWB_ERR_CUDA, "predict_pts failed") : VIWB_OK;
+}
 
 extern "C" int viwb_undistort_velocity(viwb_context *ctx, const viwb_pinhole *cam, int n, const float *pts, const float *prev_un_pts, const uint8_t *has_prev,
                                        double dt, float *un_pts, float *velocity) {
@@ -1634,6 +1672,10 @@ extern "C" int viwb_tracker_track(viwb_tracker *t, double cur_time, const uint8_
 extern "C" int viwb_tracker_download(viwb_tracker *t, int32_t *n_left, int32_t *ids, int32_t *track_cnt, float *feat, int32_t *n_right, int32_t *ids_right,
                                      float *feat_right) {
     return t ? trk_fetch(t, n_left, ids, track_cnt, feat, n_right, ids_right, feat_right) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_tracker_feedback(viwb_tracker *t, const int32_t *n_remove, const int32_t *remove_ids, const int32_t *n_pred, const int32_t *pred_ids,
+                                     const double *pred_pts_cam, const uint8_t *has_prediction) {
+    return t ? trk_feedback_run(t, n_remove, remove_ids, n_pred, pred_ids, pred_pts_cam, has_prediction) : VIWB_ERR_INVALID;
 }
 extern "C" double viwb_tracker_algorithmic_bytes(const viwb_tracker *t) {
     if (!t) return 0.0;

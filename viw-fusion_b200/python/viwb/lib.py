@@ -20,9 +20,9 @@ EXPORTS = ["viwb_create", "viwb_destroy", "viwb_last_error", "viwb_set_stream", 
            "viwb_batch_run", "viwb_batch_download", "viwb_batch_algorithmic_bytes", "viwb_batch_destroy",
            "viwb_debug_normal_equations", "viwb_lk_track", "viwb_track_checked", "viwb_lk_batch_create", "viwb_lk_batch_destroy",
            "viwb_lk_batch_upload", "viwb_lk_batch_run", "viwb_lk_batch_download", "viwb_lk_batch_algorithmic_bytes", "viwb_host_register",
-           "viwb_host_unregister", "viwb_imu_preintegrate", "viwb_wheel_preintegrate", "viwb_outlier_rejection", "viwb_batch_outliers", "viwb_triangulate", "viwb_shift_depth", "viwb_undistort_velocity",
+           "viwb_host_unregister", "viwb_imu_preintegrate", "viwb_wheel_preintegrate", "viwb_outlier_rejection", "viwb_batch_outliers", "viwb_triangulate", "viwb_shift_depth", "viwb_predict_pts", "viwb_undistort_velocity",
            "viwb_set_mask", "viwb_good_features_to_track", "viwb_detector_create", "viwb_detector_destroy", "viwb_detector_detect", "viwb_detector_algorithmic_bytes",
-           "viwb_tracker_create", "viwb_tracker_destroy", "viwb_tracker_track", "viwb_tracker_download", "viwb_tracker_algorithmic_bytes",
+           "viwb_tracker_create", "viwb_tracker_destroy", "viwb_tracker_track", "viwb_tracker_feedback", "viwb_tracker_download", "viwb_tracker_algorithmic_bytes",
            "viwb_solve_gyroscope_bias", "viwb_linear_alignment"]
 
 
@@ -277,6 +277,18 @@ class Context:
                  "viwb_shift_depth")
         return out
 
+    def predict_pts(self, state, frame_count, start_frame, num_obs, pt0, depth):
+        """Estimator::predictPtsInNextFrame over the caller's feature list -> (pts_cam [n, 3], valid [n] uint8)"""
+        st = np.ascontiguousarray(state, np.float64)
+        sf, no = np.ascontiguousarray(start_frame, np.int32), np.ascontiguousarray(num_obs, np.int32)
+        p0, dep = np.ascontiguousarray(pt0, np.float64).reshape(-1, 3), np.ascontiguousarray(depth, np.float64)
+        n = len(sf)
+        assert len(no) == n and len(p0) == n and len(dep) == n
+        out, valid = np.zeros((n, 3)), np.zeros(n, np.uint8)
+        vp = lambda x: x.ctypes.data_as(C.c_void_p)
+        self._ck(self.lib.viwb_predict_pts(self.h, _dp(st), C.c_int(frame_count), C.c_int(n), vp(sf), vp(no), _dp(p0), _dp(dep), _dp(out), vp(valid)), "viwb_predict_pts")
+        return out, valid
+
     # ---------------------------------------------------------------- pre-integration (SURVEY 8 f-2)
     @staticmethod
     def _pack_intervals(dts, a_list, b_list):
@@ -418,6 +430,26 @@ class Tracker:
         self._keep = (left, right, pl, pr, pp, hp)
         vp = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)
         self.ctx._ck(self.ctx.lib.viwb_tracker_track(self.hnd, C.c_double(cur_time), pl, pr, C.c_int(stride), vp(pp), vp(hp)), "viwb_tracker_track")
+
+    def feedback(self, remove_ids=None, predictions=None):
+        """FeatureTracker::removeOutliers then setPrediction on every stream (estimator.cpp:841-843), asynchronous.
+        remove_ids: per stream, an iterable of feature ids (or None for no removal at all).
+        predictions: per stream, None (no prediction for that stream) or (ids, pts_cam [k, 3]) -- the valid rows of Context.predict_pts;
+        the next track() consumes it and must be called without predict_pts."""
+        vp = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)
+        n_rm = rm = n_pr = pid = pts = hp = None
+        if remove_ids is not None:
+            assert len(remove_ids) == self.F
+            lists = [np.asarray(list(r) if r is not None else [], np.int32).reshape(-1) for r in remove_ids]
+            n_rm, rm = np.array([len(r) for r in lists], np.int32), np.ascontiguousarray(np.concatenate(lists), np.int32)
+        if predictions is not None:
+            assert len(predictions) == self.F
+            hp = np.array([0 if p is None else 1 for p in predictions], np.uint8)
+            idl = [np.zeros(0, np.int32) if p is None else np.asarray(p[0], np.int32).reshape(-1) for p in predictions]
+            ptl = [np.zeros((0, 3)) if p is None else np.asarray(p[1], np.float64).reshape(-1, 3) for p in predictions]
+            assert all(len(a) == len(b) for a, b in zip(idl, ptl))
+            n_pr, pid, pts = np.array([len(a) for a in idl], np.int32), np.ascontiguousarray(np.concatenate(idl), np.int32), np.ascontiguousarray(np.concatenate(ptl), np.float64)
+        self.ctx._ck(self.ctx.lib.viwb_tracker_feedback(self.hnd, vp(n_rm), vp(rm), vp(n_pr), vp(pid), vp(pts), vp(hp)), "viwb_tracker_feedback")
 
     def download(self):
         """-> per stream dicts are left to the caller; returns (n_left, ids, track_cnt, feat, n_right, ids_right, feat_right) views"""
