@@ -363,6 +363,23 @@ typedef struct viwb_pinhole { double fx, fy, cx, cy, k1, k2, p1, p2; } viwb_pinh
 int viwb_undistort_velocity(viwb_context *ctx, const viwb_pinhole *cam, int n, const float *pts, const float *prev_un_pts,
                             const uint8_t *has_prev, double dt, float *un_pts, float *velocity);
 
+/* A camera of either model camodocal builds for the reference's tracker (FeatureTracker::readIntrinsicParameter, feature_tracker.cpp):
+ *   VIWB_CAMERA_PINHOLE: p = fx fy cx cy k1 k2 p1 p2 (viwb_pinhole's order; p[8] unused), PinholeCamera.
+ *   VIWB_CAMERA_MEI:     p = xi k1 k2 p1 p2 gamma1 gamma2 u0 v0 (CataCamera's constructor and its yaml order, CataCamera.cc:300-303), the
+ *                        unified omnidirectional model with mirror parameter xi: the lift is CataCamera::liftProjective (:556-626, recursive
+ *                        distortion n = 8, distortion :766-782, m_inv_K* :319-323) and the projection CataCamera::spaceToPlane (:636-659).
+ * The MEI arithmetic is rounded operation by operation (no fused multiply-add), so its floats are the reference's bit for bit.  Parameter
+ * values are not checked, as the reference does not check them: a ray with 1 + (1 - xi^2) rho^2 < 0 lifts to NaN as it does there. */
+typedef enum { VIWB_CAMERA_PINHOLE = 0, VIWB_CAMERA_MEI = 1 } viwb_camera_model;
+typedef struct viwb_camera {
+    int32_t model;      /* viwb_camera_model */
+    double p[9];
+} viwb_camera;
+/* viwb_undistort_velocity with the lift of `cam`'s model.  An unknown model or a NULL cam is VIWB_ERR_INVALID (viwb_last_error says why).
+ * With a PINHOLE camera this is viwb_undistort_velocity, to the bit. */
+int viwb_undistort_velocity_camera(viwb_context *ctx, const viwb_camera *cam, int n, const float *pts, const float *prev_un_pts,
+                                   const uint8_t *has_prev, double dt, float *un_pts, float *velocity);
+
 /* ---- batched tracker: one camera tick of `streams` independent VIO sessions per submission --------
  * Replaces, per stream, the four calcOpticalFlowPyrLK calls of one FeatureTracker::trackImage()
  * (feature_tracker.cpp:139 temporal forward, :145-146 temporal reverse, :240 stereo forward, :244 stereo
@@ -436,6 +453,12 @@ typedef struct viwb_tracker_config {
 } viwb_tracker_config;
 typedef struct viwb_tracker viwb_tracker;
 int viwb_tracker_create(viwb_context *ctx, int streams, int width, int height, const viwb_tracker_config *config, viwb_tracker **out);
+/* viwb_tracker_create with cam[0] / cam[1] = m_camera[0] / m_camera[1] of any viwb_camera model, each camera its own (an MEI left camera
+ * beside a pinhole right camera is legal); config->cam is not read.  Both entries must name a known model, cam[1] also in a mono session,
+ * where it is not used.  The lift of undistortedPts (feature_tracker.cpp:606-617, both cameras) and setPrediction's spaceToPlane
+ * (:729, camera 0, viwb_tracker_feedback) follow each camera's model.  An unknown model or a NULL cam is VIWB_ERR_INVALID. */
+int viwb_tracker_create_camera(viwb_context *ctx, int streams, int width, int height, const viwb_tracker_config *config,
+                               const viwb_camera cam[2], viwb_tracker **out);
 void viwb_tracker_destroy(viwb_tracker *t);
 /* trackImage(cur_time, left[s], right[s]) for every stream s.  left / right: `streams` host image pointers (8-bit, `stride` bytes per
  * row; right may be NULL for a mono session).  predict_pts (optional): [streams][max_cnt][2] = FeatureTracker::setPrediction()'s
@@ -452,7 +475,7 @@ int viwb_tracker_download(viwb_tracker *t, int32_t *n_left, int32_t *ids, int32_
  * FeatureTracker::removeOutliers(remove_ids) (feature_tracker.cpp:739-755: stable reduceVector of prev_pts, ids, track_cnt; the id ->
  * undistorted point maps stay as they are) and then, for the streams with has_prediction[s] != 0, FeatureTracker::setPrediction
  * (:715-736): for each remaining row, the prediction with the row's id projected by m_camera[0]->spaceToPlane (pinhole + radtan,
- * PinholeCamera.cc:520-542) and rounded to float as cv::Point2f does, else the row's prev_pts.  The prediction stays in HBM and is
+ * PinholeCamera.cc:520-542, or MEI, CataCamera.cc:636-659) and rounded to float as cv::Point2f does, else the row's prev_pts.  The prediction stays in HBM and is
  * consumed by the next viwb_tracker_track, which must then be called with predict_pts == NULL (VIWB_ERR_INVALID otherwise, and the
  * session stays as it was); hasPrediction is cleared by that tick (:279).
  * n_remove / n_pred: [streams] list lengths; remove_ids, pred_ids: the streams' lists back to back; pred_pts_cam: [sum n_pred][3]

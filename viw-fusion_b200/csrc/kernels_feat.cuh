@@ -105,24 +105,94 @@ VIWB_D void predict_pts_item(const PredictArgs &a, int k) {
     st3(a.pts_cam + 3 * k, pts_cam);
 }
 
-// FeatureTracker::undistortedPts (featureTracker/feature_tracker.cpp:606-617) -> PinholeCamera::liftProjective with the recursive
-// distortion model, n = 8 (camera_models/src/camera_models/PinholeCamera.cc:450-517, distortion :646-662), results narrowed to
-// cv::Point2f; and FeatureTracker::ptsVelocity (:619-657) for points paired index-wise with the previous tick (SURVEY 8 f-1).
-struct UndistArgs { int n; const float *pts, *prev_un; const unsigned char *has_prev; double fx, fy, cx, cy, k1, k2, p1, p2, dt; float *un, *vel; };
-VIWB_D void undistort_item(const UndistArgs &a, int i) {
-    if (i >= a.n) return;
-    const double inv_K11 = 1.0 / a.fx, inv_K13 = -a.cx / a.fx, inv_K22 = 1.0 / a.fy, inv_K23 = -a.cy / a.fy;     // PinholeCamera.cc:105-108
-    const double mx_d = inv_K11 * (double)a.pts[2 * i] + inv_K13, my_d = inv_K22 * (double)a.pts[2 * i + 1] + inv_K23;
+// FP64 operations rounded one by one (no fused multiply-add, IEEE division and square root), so that a result is the double the
+// reference's build (-ffp-contract=off here, SSE2 there) computes, and its float narrowing the same float, bit for bit
+#ifdef VIWB_HOST_EMU
+static inline double trk_mul(double a, double b) { return a * b; }
+static inline double trk_add(double a, double b) { return a + b; }
+static inline double trk_sub(double a, double b) { return a - b; }
+static inline double trk_div(double a, double b) { return a / b; }
+static inline double trk_sqrt(double a) { return sqrt(a); }
+#else
+VIWB_D double trk_mul(double a, double b) { return __dmul_rn(a, b); }
+VIWB_D double trk_add(double a, double b) { return __dadd_rn(a, b); }
+VIWB_D double trk_sub(double a, double b) { return __dsub_rn(a, b); }
+VIWB_D double trk_div(double a, double b) { return __ddiv_rn(a, b); }
+VIWB_D double trk_sqrt(double a) { return __dsqrt_rn(a); }
+#endif
+
+// Camera models of viwb_camera (include/viwb.h).  One record holds either: PINHOLE's fx, fy, cx, cy or MEI's gamma1, gamma2, u0, v0 in
+// the same four slots (both are the K of a lift mx = (u - cx) / fx), the radtan coefficients k1, k2, p1, p2 shared by both, and MEI's xi.
+enum { CAM_PINHOLE = 0, CAM_MEI = 1 };
+struct CamModel { int model; double fx, fy, cx, cy, k1, k2, p1, p2, xi; };
+
+// CataCamera::distortion (camera_models/src/camera_models/CataCamera.cc:766-782)
+VIWB_D void mei_distortion(const CamModel &c, double x, double y, double &dx, double &dy) {
+    const double mx2 = trk_mul(x, x), my2 = trk_mul(y, y), mxy = trk_mul(x, y), rho2 = trk_add(mx2, my2);
+    const double rad = trk_add(trk_mul(c.k1, rho2), trk_mul(trk_mul(c.k2, rho2), rho2));
+    dx = trk_add(trk_add(trk_mul(x, rad), trk_mul(trk_mul(2.0, c.p1), mxy)), trk_mul(c.p2, trk_add(rho2, trk_mul(2.0, mx2))));
+    dy = trk_add(trk_add(trk_mul(y, rad), trk_mul(trk_mul(2.0, c.p2), mxy)), trk_mul(c.p1, trk_add(rho2, trk_mul(2.0, my2))));
+}
+// CataCamera::liftProjective (CataCamera.cc:556-626; m_inv_K* of :319-323, m_noDistortion of :307-317, recursive model n = 8) followed by
+// FeatureTracker::undistortedPts' b.x() / b.z(), b.y() / b.z() narrowed to cv::Point2f (featureTracker/feature_tracker.cpp:606-617).
+// A ray with 1 + (1 - xi^2) rho^2 < 0 gives NaN, one with b.z() == 0 gives inf, as in the reference.
+VIWB_D void mei_lift(const CamModel &c, float u, float v, float &x, float &y) {
+    const double inv_K11 = trk_div(1.0, c.fx), inv_K13 = trk_div(-c.cx, c.fx), inv_K22 = trk_div(1.0, c.fy), inv_K23 = trk_div(-c.cy, c.fy);
+    const double mx_d = trk_add(trk_mul(inv_K11, (double)u), inv_K13), my_d = trk_add(trk_mul(inv_K22, (double)v), inv_K23);
     double mx_u = mx_d, my_u = my_d;
-    if (!(a.k1 == 0.0 && a.k2 == 0.0 && a.p1 == 0.0 && a.p2 == 0.0)) {       // m_noDistortion
+    if (!(c.k1 == 0.0 && c.k2 == 0.0 && c.p1 == 0.0 && c.p2 == 0.0)) {
         for (int it = 0; it < 8; it++) {
-            const double x = (it == 0) ? mx_d : mx_u, y = (it == 0) ? my_d : my_u;
-            const double mx2 = x * x, my2 = y * y, mxy = x * y, rho2 = mx2 + my2, rad = a.k1 * rho2 + a.k2 * rho2 * rho2;
-            const double dx = x * rad + 2.0 * a.p1 * mxy + a.p2 * (rho2 + 2.0 * mx2), dy = y * rad + 2.0 * a.p2 * mxy + a.p1 * (rho2 + 2.0 * my2);
-            mx_u = mx_d - dx; my_u = my_d - dy;
+            double dx, dy;
+            mei_distortion(c, mx_u, my_u, dx, dy);                             // it == 0: (mx_u, my_u) == (mx_d, my_d)
+            mx_u = trk_sub(mx_d, dx); my_u = trk_sub(my_d, dy);
         }
     }
-    const float ux = (float)(mx_u / 1.0), uy = (float)(my_u / 1.0);          // b.x() / b.z() with b.z() = 1
+    double z;
+    if (c.xi == 1.0) z = trk_div(trk_sub(trk_sub(1.0, trk_mul(mx_u, mx_u)), trk_mul(my_u, my_u)), 2.0);
+    else {
+        const double rho2 = trk_add(trk_mul(mx_u, mx_u), trk_mul(my_u, my_u));
+        z = trk_sub(1.0, trk_div(trk_mul(c.xi, trk_add(rho2, 1.0)), trk_add(c.xi, trk_sqrt(trk_add(1.0, trk_mul(trk_sub(1.0, trk_mul(c.xi, c.xi)), rho2))))));
+    }
+    x = (float)trk_div(mx_u, z); y = (float)trk_div(my_u, z);
+}
+// CataCamera::spaceToPlane (CataCamera.cc:636-659) narrowed to cv::Point2f (feature_tracker.cpp:730).  |P| = sqrt((x^2 + y^2) + z^2).
+VIWB_D void mei_space_to_plane(const CamModel &c, const double *P, float &u, float &v) {
+    const double norm = trk_sqrt(trk_add(trk_add(trk_mul(P[0], P[0]), trk_mul(P[1], P[1])), trk_mul(P[2], P[2])));
+    const double z = trk_add(P[2], trk_mul(c.xi, norm));
+    double xd = trk_div(P[0], z), yd = trk_div(P[1], z);
+    if (!(c.k1 == 0.0 && c.k2 == 0.0 && c.p1 == 0.0 && c.p2 == 0.0)) {
+        double dx, dy;
+        mei_distortion(c, xd, yd, dx, dy);
+        xd = trk_add(xd, dx); yd = trk_add(yd, dy);
+    }
+    u = (float)trk_add(trk_mul(c.fx, xd), c.cx); v = (float)trk_add(trk_mul(c.fy, yd), c.cy);
+}
+
+// FeatureTracker::undistortedPts (featureTracker/feature_tracker.cpp:606-617) -> PinholeCamera::liftProjective with the recursive
+// distortion model, n = 8 (camera_models/src/camera_models/PinholeCamera.cc:450-517, distortion :646-662), results narrowed to
+// cv::Point2f, or mei_lift when model == CAM_MEI; and FeatureTracker::ptsVelocity (:619-657) for points paired index-wise with the
+// previous tick (SURVEY 8 f-1).
+struct UndistArgs { int n; const float *pts, *prev_un; const unsigned char *has_prev; double fx, fy, cx, cy, k1, k2, p1, p2, dt; float *un, *vel; int model; double xi; };
+VIWB_D void undistort_item(const UndistArgs &a, int i) {
+    if (i >= a.n) return;
+    float ux, uy;
+    if (a.model == CAM_MEI) {
+        const CamModel c = {a.model, a.fx, a.fy, a.cx, a.cy, a.k1, a.k2, a.p1, a.p2, a.xi};
+        mei_lift(c, a.pts[2 * i], a.pts[2 * i + 1], ux, uy);
+    } else {                                                                // the pinhole lift keeps its contracted arithmetic (2e-7 bar)
+        const double inv_K11 = 1.0 / a.fx, inv_K13 = -a.cx / a.fx, inv_K22 = 1.0 / a.fy, inv_K23 = -a.cy / a.fy;     // PinholeCamera.cc:105-108
+        const double mx_d = inv_K11 * (double)a.pts[2 * i] + inv_K13, my_d = inv_K22 * (double)a.pts[2 * i + 1] + inv_K23;
+        double mx_u = mx_d, my_u = my_d;
+        if (!(a.k1 == 0.0 && a.k2 == 0.0 && a.p1 == 0.0 && a.p2 == 0.0)) {       // m_noDistortion
+            for (int it = 0; it < 8; it++) {
+                const double x = (it == 0) ? mx_d : mx_u, y = (it == 0) ? my_d : my_u;
+                const double mx2 = x * x, my2 = y * y, mxy = x * y, rho2 = mx2 + my2, rad = a.k1 * rho2 + a.k2 * rho2 * rho2;
+                const double dx = x * rad + 2.0 * a.p1 * mxy + a.p2 * (rho2 + 2.0 * mx2), dy = y * rad + 2.0 * a.p2 * mxy + a.p1 * (rho2 + 2.0 * my2);
+                mx_u = mx_d - dx; my_u = my_d - dy;
+            }
+        }
+        ux = (float)(mx_u / 1.0); uy = (float)(my_u / 1.0);                     // b.x() / b.z() with b.z() = 1
+    }
     a.un[2 * i] = ux; a.un[2 * i + 1] = uy;
     if (a.vel) {
         float vx = 0.f, vy = 0.f;

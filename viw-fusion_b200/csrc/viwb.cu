@@ -1567,6 +1567,15 @@ extern "C" int viwb_predict_pts(viwb_context *ctx, const double *state, int fram
 extern "C" int viwb_undistort_velocity(viwb_context *ctx, const viwb_pinhole *cam, int n, const float *pts, const float *prev_un_pts, const uint8_t *has_prev,
                                        double dt, float *un_pts, float *velocity) {
     if (!ctx || !cam || n < 0 || !pts || !un_pts) return VIWB_ERR_INVALID;
+    const viwb_camera c = pinhole_camera(*cam);
+    return viwb_undistort_velocity_camera(ctx, &c, n, pts, prev_un_pts, has_prev, dt, un_pts, velocity);
+}
+
+extern "C" int viwb_undistort_velocity_camera(viwb_context *ctx, const viwb_camera *cam, int n, const float *pts, const float *prev_un_pts, const uint8_t *has_prev,
+                                              double dt, float *un_pts, float *velocity) {
+    if (!ctx || n < 0 || !pts || !un_pts) return VIWB_ERR_INVALID;
+    CamModel cm;
+    if (camera_model(ctx, cam, &cm)) return VIWB_ERR_INVALID;
     if (n == 0) return VIWB_OK;
     bind_device(ctx);
     const size_t pb = align_up((size_t)n * 8);
@@ -1577,7 +1586,7 @@ extern "C" int viwb_undistort_velocity(viwb_context *ctx, const viwb_pinhole *ca
     if (!e && prev_un_pts) e = dev_h2d(d_prev, prev_un_pts, (size_t)n * 8, ctx->stream);
     if (!e && has_prev) e = dev_h2d(d_hp, has_prev, (size_t)n, ctx->stream);
     UndistArgs a; a.n = n; a.pts = d_pts; a.prev_un = prev_un_pts ? d_prev : nullptr; a.has_prev = has_prev ? d_hp : nullptr;
-    a.fx = cam->fx; a.fy = cam->fy; a.cx = cam->cx; a.cy = cam->cy; a.k1 = cam->k1; a.k2 = cam->k2; a.p1 = cam->p1; a.p2 = cam->p2; a.dt = dt;
+    a.fx = cm.fx; a.fy = cm.fy; a.cx = cm.cx; a.cy = cm.cy; a.k1 = cm.k1; a.k2 = cm.k2; a.p1 = cm.p1; a.p2 = cm.p2; a.dt = dt; a.model = cm.model; a.xi = cm.xi;
     a.un = d_un; a.vel = velocity ? d_vel : nullptr;
     if (!e) {
 #ifdef VIWB_HOST_EMU
@@ -1659,7 +1668,15 @@ extern "C" double viwb_lk_batch_algorithmic_bytes(const viwb_lk_batch *b) {
 extern "C" int viwb_tracker_create(viwb_context *ctx, int streams, int width, int height, const viwb_tracker_config *config, viwb_tracker **out) {
     if (!ctx || !out) return VIWB_ERR_INVALID;
     if (width < 3 || height < 3) return fail(ctx, VIWB_ERR_INVALID, "tracker: bad image size");
-    return trk_build(ctx, streams, width, height, config, out);
+    viwb_camera cam[2] = {};
+    if (config) for (int c = 0; c < 2; c++) cam[c] = pinhole_camera(config->cam[c]);
+    return trk_build(ctx, streams, width, height, config, cam, out);
+}
+extern "C" int viwb_tracker_create_camera(viwb_context *ctx, int streams, int width, int height, const viwb_tracker_config *config, const viwb_camera cam[2],
+                                          viwb_tracker **out) {
+    if (!ctx || !out) return VIWB_ERR_INVALID;
+    if (width < 3 || height < 3) return fail(ctx, VIWB_ERR_INVALID, "tracker: bad image size");
+    return trk_build(ctx, streams, width, height, config, cam, out);
 }
 extern "C" void viwb_tracker_destroy(viwb_tracker *t) { trk_free(t); }
 extern "C" int viwb_tracker_track(viwb_tracker *t, double cur_time, const uint8_t *const *left, const uint8_t *const *right, int stride, const float *predict_pts,

@@ -20,9 +20,9 @@ EXPORTS = ["viwb_create", "viwb_destroy", "viwb_last_error", "viwb_set_stream", 
            "viwb_batch_run", "viwb_batch_download", "viwb_batch_algorithmic_bytes", "viwb_batch_destroy",
            "viwb_debug_normal_equations", "viwb_lk_track", "viwb_track_checked", "viwb_lk_batch_create", "viwb_lk_batch_destroy",
            "viwb_lk_batch_upload", "viwb_lk_batch_run", "viwb_lk_batch_download", "viwb_lk_batch_algorithmic_bytes", "viwb_host_register",
-           "viwb_host_unregister", "viwb_imu_preintegrate", "viwb_wheel_preintegrate", "viwb_outlier_rejection", "viwb_batch_outliers", "viwb_triangulate", "viwb_shift_depth", "viwb_predict_pts", "viwb_undistort_velocity",
+           "viwb_host_unregister", "viwb_imu_preintegrate", "viwb_wheel_preintegrate", "viwb_outlier_rejection", "viwb_batch_outliers", "viwb_triangulate", "viwb_shift_depth", "viwb_predict_pts", "viwb_undistort_velocity", "viwb_undistort_velocity_camera",
            "viwb_set_mask", "viwb_good_features_to_track", "viwb_detector_create", "viwb_detector_destroy", "viwb_detector_detect", "viwb_detector_algorithmic_bytes",
-           "viwb_tracker_create", "viwb_tracker_destroy", "viwb_tracker_track", "viwb_tracker_feedback", "viwb_tracker_download", "viwb_tracker_algorithmic_bytes",
+           "viwb_tracker_create", "viwb_tracker_create_camera", "viwb_tracker_destroy", "viwb_tracker_track", "viwb_tracker_feedback", "viwb_tracker_download", "viwb_tracker_algorithmic_bytes",
            "viwb_solve_gyroscope_bias", "viwb_linear_alignment"]
 
 
@@ -248,16 +248,19 @@ class Context:
         return out[: problem.num_landmarks]
 
     def undistort_velocity(self, cam, pts, prev_un=None, has_prev=None, dt=0.05, want_velocity=True):
-        """cam = (fx, fy, cx, cy, k1, k2, p1, p2); pts float32 (n, 2) pixels -> (normalised points, velocities) as float32"""
+        """cam = (fx, fy, cx, cy, k1, k2, p1, p2) (viwb_undistort_velocity) or a Camera of either model (viwb_undistort_velocity_camera);
+        pts float32 (n, 2) pixels -> (normalised points, velocities) as float32"""
         p = np.ascontiguousarray(pts, np.float32).reshape(-1, 2)
         n = len(p)
-        c = (C.c_double * 8)(*[float(v) for v in cam])
         un, vel = np.zeros((n, 2), np.float32), np.zeros((n, 2), np.float32)
         pv = None if prev_un is None else np.ascontiguousarray(prev_un, np.float32)
         hp = None if has_prev is None else np.ascontiguousarray(has_prev, np.uint8)
         vp = lambda x: None if x is None else x.ctypes.data_as(C.c_void_p)
-        self._ck(self.lib.viwb_undistort_velocity(self.h, c, C.c_int(n), vp(p), vp(pv), vp(hp), C.c_double(dt), vp(un), vp(vel) if want_velocity else None),
-                 "viwb_undistort_velocity")
+        if isinstance(cam, Camera):
+            fn, name, c = self.lib.viwb_undistort_velocity_camera, "viwb_undistort_velocity_camera", C.byref(cam)
+        else:
+            fn, name, c = self.lib.viwb_undistort_velocity, "viwb_undistort_velocity", (C.c_double * 8)(*[float(v) for v in cam])
+        self._ck(fn(self.h, c, C.c_int(n), vp(p), vp(pv), vp(hp), C.c_double(dt), vp(un), vp(vel) if want_velocity else None), name)
         return un, vel
 
     def triangulate(self, state, stereo, frame, pt0, pt1, init_depth=5.0):
@@ -394,20 +397,44 @@ class Context:
         self._ck(self.lib.viwb_host_unregister(self.h, C.c_void_p(arr.ctypes.data)), "viwb_host_unregister")
 
 
+CAMERA_PINHOLE, CAMERA_MEI = 0, 1
+
+
+class Camera(C.Structure):
+    """viwb_camera: a camera of either model (include/viwb.h).  Build one with Camera.pinhole(...) or Camera.mei(...)."""
+    _fields_ = [("model", C.c_int32), ("p", C.c_double * 9)]
+
+    @classmethod
+    def pinhole(cls, fx, fy, cx, cy, k1, k2, p1, p2):
+        return cls(CAMERA_PINHOLE, (C.c_double * 9)(fx, fy, cx, cy, k1, k2, p1, p2, 0.0))
+
+    @classmethod
+    def mei(cls, xi, k1, k2, p1, p2, gamma1, gamma2, u0, v0):
+        """the parameters in the order of a camodocal MEI yaml file (CataCamera's constructor)"""
+        return cls(CAMERA_MEI, (C.c_double * 9)(xi, k1, k2, p1, p2, gamma1, gamma2, u0, v0))
+
+
 class TrackerConfig(C.Structure):
     _fields_ = [("max_cnt", C.c_int), ("min_dist", C.c_int), ("flow_back", C.c_int), ("stereo", C.c_int), ("cam", C.c_double * 16)]
 
 
 class Tracker:
     """`streams` FeatureTracker sessions resident on the device (viwb_tracker_*): track() = FeatureTracker::trackImage() per stream.
-    cam0 / cam1 = (fx, fy, cx, cy, k1, k2, p1, p2); cam1 None = mono sessions."""
+    cam0 / cam1 = (fx, fy, cx, cy, k1, k2, p1, p2) (viwb_tracker_create) or, when either is a Camera, cameras of any model
+    (viwb_tracker_create_camera; a tuple beside a Camera is taken as a pinhole Camera); cam1 None = mono sessions."""
 
     def __init__(self, ctx, streams, width, height, cam0, cam1=None, max_cnt=150, min_dist=30, flow_back=True):
         self.ctx, self.F, self.w, self.h, self.maxn, self.stereo = ctx, streams, width, height, max_cnt, cam1 is not None
-        cfg = TrackerConfig(max_cnt, int(min_dist), 1 if flow_back else 0, 1 if self.stereo else 0,
-                            (C.c_double * 16)(*([float(v) for v in cam0] + [float(v) for v in (cam1 if cam1 is not None else cam0)])))
         self.hnd = C.c_void_p()
-        ctx._ck(ctx.lib.viwb_tracker_create(ctx.h, C.c_int(streams), C.c_int(width), C.c_int(height), C.byref(cfg), C.byref(self.hnd)), "viwb_tracker_create")
+        if isinstance(cam0, Camera) or isinstance(cam1, Camera):
+            cams = [c if isinstance(c, Camera) else Camera.pinhole(*[float(v) for v in c]) for c in (cam0, cam1 if cam1 is not None else cam0)]
+            cfg = TrackerConfig(max_cnt, int(min_dist), 1 if flow_back else 0, 1 if self.stereo else 0)
+            ctx._ck(ctx.lib.viwb_tracker_create_camera(ctx.h, C.c_int(streams), C.c_int(width), C.c_int(height), C.byref(cfg), (Camera * 2)(*cams), C.byref(self.hnd)),
+                    "viwb_tracker_create_camera")
+        else:
+            cfg = TrackerConfig(max_cnt, int(min_dist), 1 if flow_back else 0, 1 if self.stereo else 0,
+                                (C.c_double * 16)(*([float(v) for v in cam0] + [float(v) for v in (cam1 if cam1 is not None else cam0)])))
+            ctx._ck(ctx.lib.viwb_tracker_create(ctx.h, C.c_int(streams), C.c_int(width), C.c_int(height), C.byref(cfg), C.byref(self.hnd)), "viwb_tracker_create")
         self.n_left, self.n_right = np.zeros(streams, np.int32), np.zeros(streams, np.int32)
         self.ids, self.track_cnt, self.ids_right = (np.zeros((streams, max_cnt), np.int32) for _ in range(3))
         self.feat, self.feat_right = np.zeros((streams, max_cnt, 6), np.float32), np.zeros((streams, max_cnt, 6), np.float32)
