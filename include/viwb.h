@@ -490,6 +490,90 @@ int viwb_tracker_feedback(viwb_tracker *t, const int32_t *n_remove, const int32_
 /* compulsory HBM bytes of one tick: the new images read once by the pyramid and once by the detector, pyramid levels written, rows out */
 double viwb_tracker_algorithmic_bytes(const viwb_tracker *t);
 
+/* ---- resident FeatureManager: estimator/feature_manager.{h,cpp} for `streams` independent sessions ----------------------------------------
+ * The NON_LINEAR branch of Estimator::processImage (estimator.cpp:690-878) around the solve, per stream and without a host round trip:
+ *   add (+ decisions)   f_manager.addFeatureCheckParallax (:694-703; feature_manager.cpp:52-119, compensatedParallax2 :538-571)
+ *   triangulate         f_manager.triangulate (:832; feature_manager.cpp:309-389, the two live branches)
+ *   window              the visual-factor loop of optimization() (:1585-1638) and getDepthVector (feature_manager.cpp:179-195)
+ *   set_depth           double2vector's f_manager.setDepth (:1324-1327; feature_manager.cpp:142-160)
+ *   remove_outliers     f_manager.removeOutlier(removeIndex) (:835-837; feature_manager.cpp:440-455)
+ *   predict             predictPtsInNextFrame (:2080-2113)
+ *   slide               slideWindowOld / slideWindowNew's FeatureManager part (:1898-2063; feature_manager.cpp:457-536)
+ *   remove_failures     f_manager.removeFailures (:859; feature_manager.cpp:162-171)
+ * Each stream's list keeps the reference's order: insertion order (new ids appended in ascending id order, as the image map iterates),
+ * stable erasures; an id erased and then seen again is appended as a new feature.  The landmark numbering of a window export is that order
+ * filtered by num_obs >= 4.  Observations are stored as the six floats {x, y, p_u, p_v, v_x, v_y} per camera (z = 1) and the double cur_td:
+ * every featureFrame producer of the reference takes its numbers from floats, so these reproduce FeaturePerFrame exactly.
+ * Per-stream host arrays lie back to back with fixed strides.  Every call launches the same number of kernels whatever `streams` is; calls
+ * that return data synchronise, the others are asynchronous on the context stream. */
+typedef struct viwb_features_config {
+    int max_rows;          /* featureFrame rows per stream and tick (MAX_CNT), <= 1024; a tracker fed to add_tracked needs max_cnt <= max_rows */
+    int max_features;      /* list capacity per stream; 0 = (VIWB_WINDOW_SIZE + 1) * max_rows, which valid input cannot exceed */
+    int stereo;            /* STEREO */
+    double min_parallax;   /* MIN_PARALLAX = keyframe_parallax / FOCAL_LENGTH (parameters.cpp:267-268) */
+    double focal_length;   /* FOCAL_LENGTH (460); only last_average_parallax uses it */
+    double init_depth;     /* INIT_DEPTH (5.0) */
+} viwb_features_config;
+typedef struct viwb_features viwb_features;
+int viwb_features_create(viwb_context *ctx, int streams, const viwb_features_config *config, viwb_features **out);
+void viwb_features_destroy(viwb_features *fs);
+/* addFeatureCheckParallax(frame_count[s], image, td[s]) per stream, the image map built from host rows in viwb_tracker_download's layout
+ * with max_rows as the stride: n_left [streams], ids [streams][max_rows], feat [streams][max_rows][6], and the right camera's rows (n_right
+ * NULL or a mono configuration: none).  A duplicate left or right id, a right id without a left row (the reference asserts, :65-70), a row
+ * count outside [0, max_rows] or a frame_count outside [0, VIWB_WINDOW_SIZE] returns VIWB_ERR_INVALID at once and nothing is queued.  A list
+ * that would exceed max_features or a feature that would get a twelfth observation is found on the device: then no list changes and the
+ * next synchronising call (decisions, window, remove_outliers, predict, download) returns VIWB_ERR_INVALID naming the stream, and does
+ * nothing else.  Such an error stays set on the device until that call reads it: an add queued behind a failed one changes no list either,
+ * so no failure is ever overwritten and no frame is skipped silently.  The decisions stay those of the last add that was applied. */
+int viwb_features_add(viwb_features *fs, const int32_t *frame_count, const double *td, const int32_t *n_left, const int32_t *ids, const float *feat,
+                      const int32_t *n_right, const int32_t *ids_right, const float *feat_right);
+/* The same with the rows of the last tick of `t` read in HBM: no row crosses the bus.  t must belong to the same context and have the same
+ * stream count (else VIWB_ERR_INVALID at once).  The row rules above are checked on the device.  A stream whose tick overflowed
+ * goodFeaturesToTrack's candidate list is not consumed (its list stays as it was, the other streams are added) and the next synchronising
+ * call reports it; until then later adds leave that stream's list alone too. */
+int viwb_features_add_tracked(viwb_features *fs, const viwb_tracker *t, const int32_t *frame_count, const double *td);
+/* The verdicts of the last add, [streams] each (any pointer may be NULL): margin_flag = VIWB_MARGIN_OLD (keyframe) or VIWB_MARGIN_SECOND_NEW,
+ * last_track_num, long_track_num (a feature counts when it has >= 4 observations after the push), new_feature_num, last_average_parallax
+ * (0 unless the parallax branch ran).  Synchronises. */
+int viwb_features_decisions(viwb_features *fs, int32_t *margin_flag, int32_t *last_track_num, int32_t *long_track_num, int32_t *new_feature_num,
+                            double *last_average_parallax);
+/* f_manager.triangulate(frame_count, Ps, Rs, tic, ric) on every stream: states [streams][VIWB_STATE_FIXED] (poses and extrinsics as in
+ * viwb_problem's state).  Per feature the function of viwb_triangulate, so a depth is the one viwb_triangulate gives on the downloaded list. */
+int viwb_features_triangulate(viwb_features *fs, const double *states);
+/* The visual table of every stream in viwb_problem's layout (estimator.cpp:1585-1638): rows [streams][vis_cap] of vis_type / vis_landmark /
+ * vis_frame_i / vis_frame_j (imu_j; == vis_frame_i for 1F2C) / vis_obs [12], num_vis [streams]; landmark k's inverse depth (getDepthVector,
+ * 1 / estimated_depth) and feature id in [streams][VIWB_MAX_LANDMARKS], num_landmarks [streams].  The doubles are the stored floats and
+ * cur_td, so the table is exact.  More than VIWB_MAX_LANDMARKS landmarks or more than vis_cap rows in a stream is VIWB_ERR_INVALID naming
+ * it.  The export's numbering is what set_depth and remove_outliers take.  Synchronises. */
+int viwb_features_window(viwb_features *fs, int vis_cap, int32_t *num_landmarks, int32_t *num_vis, int32_t *vis_type, int32_t *vis_landmark,
+                         int32_t *vis_frame_i, int32_t *vis_frame_j, double *vis_obs, double *inv_depth, int32_t *landmark_ids);
+/* setDepth: landmark k's estimated_depth = 1.0 / inv_depth[s][k] and solve_flag = 2 if negative else 1.  VIWB_ERR_INVALID if a list changed
+ * (add, remove_outliers, slide, remove_failures) since the last export. */
+int viwb_features_set_depth(viwb_features *fs, const double *inv_depth /* [streams][VIWB_MAX_LANDMARKS] */);
+/* removeOutlier with per-landmark verdicts in the numbering of the last export (what viwb_batch_outliers / viwb_outlier_rejection produce);
+ * the removed ids of each stream in ascending order (std::set order), ready for viwb_tracker_feedback.  VIWB_ERR_INVALID if a list changed
+ * since the last export.  Synchronises. */
+int viwb_features_remove_outliers(viwb_features *fs, const uint8_t *outliers /* [streams][VIWB_MAX_LANDMARKS] */, int32_t *n_removed,
+                                  int32_t *removed_ids /* [streams][max_features] */);
+/* predictPtsInNextFrame over the resident lists (the function of viwb_predict_pts), compacted to the features it inserts, in list order and
+ * the streams back to back: n_pred [streams], pred_ids / pred_pts_cam [sum n_pred] / [sum n_pred][3] (capacity streams * max_features),
+ * has_prediction [streams] = frame_count >= 2 (:2083 returns before setPrediction) -- viwb_tracker_feedback's arguments.  Synchronises. */
+int viwb_features_predict(viwb_features *fs, const double *states, const int32_t *frame_count, int32_t *n_pred, int32_t *pred_ids,
+                          double *pred_pts_cam, uint8_t *has_prediction);
+/* slideWindow's FeatureManager part with the margin flag of the last add; a stream with frame_count != VIWB_WINDOW_SIZE is left alone.
+ * MARGIN_OLD: shift_depth[s] (solver_flag == NON_LINEAR) -> removeBackShiftDepth(marg_R, marg_P, new_R, new_P) with the camera poses of
+ * slideWindowOld (:2053-2059; R row-major [streams][9], P [streams][3]; may be NULL when no shift_depth[s] is set), else removeBack.
+ * MARGIN_SECOND_NEW: removeFront(frame_count), including its missing depth shift (feature_manager.cpp:533). */
+int viwb_features_slide(viwb_features *fs, const int32_t *frame_count, const uint8_t *shift_depth, const double *marg_R, const double *marg_P,
+                        const double *new_R, const double *new_P);
+/* removeFailures: erase every feature with solve_flag == 2 */
+int viwb_features_remove_failures(viwb_features *fs);
+/* The lists as they stand (tests, PnP initialisation on the host, debugging): n [streams]; [streams][max_features] ids, start_frame, num_obs,
+ * depth, solve_flag; obs [streams][max_features][11][12] floats (left x y p_u p_v v_x v_y, then the right camera's, 0 without one), cur_td
+ * [..][11], is_stereo [..][11].  Entries past n[s] or num_obs are undefined.  Any pointer may be NULL.  Synchronises. */
+int viwb_features_download(viwb_features *fs, int32_t *n, int32_t *ids, int32_t *start_frame, int32_t *num_obs, double *depth, int32_t *solve_flag,
+                           float *obs, double *cur_td, uint8_t *is_stereo);
+
 /* Page-lock / unlock caller-owned host memory (camera frame buffers) for asynchronous full-rate uploads. */
 int viwb_host_register(viwb_context *ctx, void *ptr, size_t bytes);
 int viwb_host_unregister(viwb_context *ctx, void *ptr);

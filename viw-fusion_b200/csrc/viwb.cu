@@ -16,6 +16,7 @@
 #include "kernels_init.cuh"
 #include "kernels_detect.cuh"
 #include "kernels_track.cuh"
+#include "kernels_fm.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -174,6 +175,7 @@ static inline void bind_device(const viwb_context *ctx) {
 #include "lk_host.inl"
 #include "detect_host.inl"
 #include "track_host.inl"
+#include "features_host.inl"
 
 // ====================================================================================== batch
 struct HostPrior { int valid, n, nb; int block_id[NB], block_idx[NB]; std::vector<double> x0, J, r; };
@@ -1701,6 +1703,46 @@ extern "C" double viwb_tracker_algorithmic_bytes(const viwb_tracker *t) {
     const double img = (double)t->w * t->h, cams = t->stereo ? 2.0 : 1.0;
     return (double)t->F * (cams * (img + px) + img + (double)t->maxn * (cams * (24 + 4) + 4));
 }
+// -------------------------------------------------------------------------------------- resident FeatureManager (features_host.inl)
+extern "C" int viwb_features_create(viwb_context *ctx, int streams, const viwb_features_config *config, viwb_features **out) {
+    if (!ctx || !out) return VIWB_ERR_INVALID;
+    return fm_build(ctx, streams, config, out);
+}
+extern "C" void viwb_features_destroy(viwb_features *fs) { fm_free(fs); }
+extern "C" int viwb_features_add(viwb_features *fs, const int32_t *frame_count, const double *td, const int32_t *n_left, const int32_t *ids, const float *feat,
+                                 const int32_t *n_right, const int32_t *ids_right, const float *feat_right) {
+    return fs ? fm_add_host(fs, frame_count, td, n_left, ids, feat, n_right, ids_right, feat_right) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_add_tracked(viwb_features *fs, const viwb_tracker *t, const int32_t *frame_count, const double *td) {
+    return fs ? fm_add_tracked(fs, t, frame_count, td) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_decisions(viwb_features *fs, int32_t *margin_flag, int32_t *last_track_num, int32_t *long_track_num, int32_t *new_feature_num,
+                                       double *last_average_parallax) {
+    return fs ? fm_decisions(fs, margin_flag, last_track_num, long_track_num, new_feature_num, last_average_parallax) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_triangulate(viwb_features *fs, const double *states) { return fs ? fm_triangulate_run(fs, states) : VIWB_ERR_INVALID; }
+extern "C" int viwb_features_window(viwb_features *fs, int vis_cap, int32_t *num_landmarks, int32_t *num_vis, int32_t *vis_type, int32_t *vis_landmark,
+                                    int32_t *vis_frame_i, int32_t *vis_frame_j, double *vis_obs, double *inv_depth, int32_t *landmark_ids) {
+    return fs ? fm_window(fs, vis_cap, num_landmarks, num_vis, vis_type, vis_landmark, vis_frame_i, vis_frame_j, vis_obs, inv_depth, landmark_ids) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_set_depth(viwb_features *fs, const double *inv_depth) { return fs ? fm_set_depth_run(fs, inv_depth) : VIWB_ERR_INVALID; }
+extern "C" int viwb_features_remove_outliers(viwb_features *fs, const uint8_t *outliers, int32_t *n_removed, int32_t *removed_ids) {
+    return fs ? fm_remove_outliers(fs, outliers, n_removed, removed_ids) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_predict(viwb_features *fs, const double *states, const int32_t *frame_count, int32_t *n_pred, int32_t *pred_ids, double *pred_pts_cam,
+                                     uint8_t *has_prediction) {
+    return fs ? fm_predict_run(fs, states, frame_count, n_pred, pred_ids, pred_pts_cam, has_prediction) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_slide(viwb_features *fs, const int32_t *frame_count, const uint8_t *shift_depth, const double *marg_R, const double *marg_P,
+                                   const double *new_R, const double *new_P) {
+    return fs ? fm_slide(fs, frame_count, shift_depth, marg_R, marg_P, new_R, new_P) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_remove_failures(viwb_features *fs) { return fs ? fm_remove_failures(fs) : VIWB_ERR_INVALID; }
+extern "C" int viwb_features_download(viwb_features *fs, int32_t *n, int32_t *ids, int32_t *start_frame, int32_t *num_obs, double *depth, int32_t *solve_flag,
+                                      float *obs, double *cur_td, uint8_t *is_stereo) {
+    return fs ? fm_download(fs, n, ids, start_frame, num_obs, depth, solve_flag, obs, cur_td, is_stereo) : VIWB_ERR_INVALID;
+}
+
 extern "C" int viwb_host_register(viwb_context *ctx, void *ptr, size_t bytes) {
     bind_device(ctx);
     if (!ctx || !ptr) return VIWB_ERR_INVALID;

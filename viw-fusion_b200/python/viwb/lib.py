@@ -23,7 +23,10 @@ EXPORTS = ["viwb_create", "viwb_destroy", "viwb_last_error", "viwb_set_stream", 
            "viwb_host_unregister", "viwb_imu_preintegrate", "viwb_wheel_preintegrate", "viwb_outlier_rejection", "viwb_batch_outliers", "viwb_triangulate", "viwb_shift_depth", "viwb_predict_pts", "viwb_undistort_velocity", "viwb_undistort_velocity_camera",
            "viwb_set_mask", "viwb_good_features_to_track", "viwb_detector_create", "viwb_detector_destroy", "viwb_detector_detect", "viwb_detector_algorithmic_bytes",
            "viwb_tracker_create", "viwb_tracker_create_camera", "viwb_tracker_destroy", "viwb_tracker_track", "viwb_tracker_feedback", "viwb_tracker_download", "viwb_tracker_algorithmic_bytes",
-           "viwb_solve_gyroscope_bias", "viwb_linear_alignment"]
+           "viwb_solve_gyroscope_bias", "viwb_linear_alignment",
+           "viwb_features_create", "viwb_features_destroy", "viwb_features_add", "viwb_features_add_tracked", "viwb_features_decisions", "viwb_features_triangulate",
+           "viwb_features_window", "viwb_features_set_depth", "viwb_features_remove_outliers", "viwb_features_predict", "viwb_features_slide",
+           "viwb_features_remove_failures", "viwb_features_download"]
 
 
 class ViwbError(RuntimeError):
@@ -50,6 +53,8 @@ def load(libpath=None):
     lib.viwb_tracker_algorithmic_bytes.argtypes = [C.c_void_p]
     lib.viwb_tracker_destroy.argtypes = [C.c_void_p]
     lib.viwb_tracker_destroy.restype = None
+    lib.viwb_features_destroy.argtypes = [C.c_void_p]
+    lib.viwb_features_destroy.restype = None
     return lib
 
 
@@ -390,6 +395,9 @@ class Context:
     def tracker(self, streams, width, height, cam0, cam1=None, max_cnt=150, min_dist=30, flow_back=True):
         return Tracker(self, streams, width, height, cam0, cam1, max_cnt, min_dist, flow_back)
 
+    def features(self, streams, max_rows, stereo, min_parallax, focal_length=460.0, init_depth=5.0, max_features=0):
+        return Features(self, streams, max_rows, stereo, min_parallax, focal_length, init_depth, max_features)
+
     def host_register(self, arr):
         self._ck(self.lib.viwb_host_register(self.h, C.c_void_p(arr.ctypes.data), C.c_size_t(arr.nbytes)), "viwb_host_register")
 
@@ -398,6 +406,7 @@ class Context:
 
 
 CAMERA_PINHOLE, CAMERA_MEI = 0, 1
+MAX_LANDMARKS = 1000          # VIWB_MAX_LANDMARKS, the per-stream landmark stride of the viwb_features_* arrays
 
 
 class Camera(C.Structure):
@@ -503,6 +512,140 @@ class Tracker:
     def close(self):
         if self.hnd:
             self.ctx.lib.viwb_tracker_destroy(self.hnd)
+            self.hnd = C.c_void_p()
+
+
+class FeaturesConfig(C.Structure):
+    _fields_ = [("max_rows", C.c_int), ("max_features", C.c_int), ("stereo", C.c_int), ("min_parallax", C.c_double), ("focal_length", C.c_double),
+                ("init_depth", C.c_double)]
+
+
+class Features:
+    """`streams` FeatureManager lists resident on the device (viwb_features_*).  Per-stream arguments are sequences / arrays of length streams;
+    states are [streams, 207] windows.  Errors raise ViwbError."""
+
+    def __init__(self, ctx, streams, max_rows, stereo, min_parallax, focal_length=460.0, init_depth=5.0, max_features=0):
+        self.ctx, self.F, self.R, self.stereo = ctx, streams, max_rows, bool(stereo)
+        self.M = max_features or (abi.NUM_FRAMES * max_rows)
+        self.hnd = C.c_void_p()
+        cfg = FeaturesConfig(max_rows, max_features, 1 if stereo else 0, min_parallax, focal_length, init_depth)
+        ctx._ck(ctx.lib.viwb_features_create(ctx.h, C.c_int(streams), C.byref(cfg), C.byref(self.hnd)), "viwb_features_create")
+
+    def _call(self, name, *args):
+        self.ctx._ck(getattr(self.ctx.lib, name)(self.hnd, *args), name)
+
+    @staticmethod
+    def _vp(x):
+        return None if x is None else x.ctypes.data_as(C.c_void_p)
+
+    def _per_stream(self, v, dtype):
+        a = np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype), (self.F,)), dtype)
+        return a
+
+    def add(self, frame_count, td, rows):
+        """rows: per stream (ids, feat [n, 6]) or (ids, feat, ids_right, feat_right) -- the featureFrame of the tick"""
+        R, F = self.R, self.F
+        nl, nr = np.zeros(F, np.int32), np.zeros(F, np.int32)
+        ids, idr = np.zeros((F, R), np.int32), np.zeros((F, R), np.int32)
+        feat, fr = np.zeros((F, R, 6), np.float32), np.zeros((F, R, 6), np.float32)
+        for s, row in enumerate(rows):
+            a, b = np.asarray(row[0], np.int32).reshape(-1), np.asarray(row[1], np.float32).reshape(-1, 6)
+            nl[s] = len(a)
+            ids[s, : min(len(a), R)], feat[s, : min(len(a), R)] = a[:R], b[:R]
+            if len(row) > 2 and row[2] is not None:
+                c, d = np.asarray(row[2], np.int32).reshape(-1), np.asarray(row[3], np.float32).reshape(-1, 6)
+                nr[s] = len(c)
+                idr[s, : min(len(c), R)], fr[s, : min(len(c), R)] = c[:R], d[:R]
+        fc, t = self._per_stream(frame_count, np.int32), self._per_stream(td, np.float64)
+        vp = self._vp
+        self._call("viwb_features_add", vp(fc), vp(t), vp(nl), vp(ids), vp(feat), vp(nr) if self.stereo else None, vp(idr), vp(fr))
+
+    def add_tracked(self, tracker, frame_count, td):
+        fc, t = self._per_stream(frame_count, np.int32), self._per_stream(td, np.float64)
+        self._call("viwb_features_add_tracked", tracker.hnd, self._vp(fc), self._vp(t))
+
+    def decisions(self):
+        """-> dict of [streams] arrays: margin_flag, last_track_num, long_track_num, new_feature_num, last_average_parallax"""
+        out = {k: np.zeros(self.F, np.int32) for k in ("margin_flag", "last_track_num", "long_track_num", "new_feature_num")}
+        out["last_average_parallax"] = np.zeros(self.F)
+        vp = self._vp
+        self._call("viwb_features_decisions", vp(out["margin_flag"]), vp(out["last_track_num"]), vp(out["long_track_num"]), vp(out["new_feature_num"]),
+                   vp(out["last_average_parallax"]))
+        return out
+
+    def triangulate(self, states):
+        st = np.ascontiguousarray(states, np.float64).reshape(self.F, abi.STATE_FIXED)
+        self._call("viwb_features_triangulate", self._vp(st))
+
+    def window(self, vis_cap):
+        """-> (tables, inv_depth, landmark_ids): tables[s] = the visual keyword arguments of abi.WindowProblem (num_landmarks, vis_type,
+        vis_landmark, vis_frame_i, vis_frame_j, vis_obs); inv_depth[s] / landmark_ids[s] per landmark"""
+        F, L = self.F, MAX_LANDMARKS
+        nlm, nv = np.zeros(F, np.int32), np.zeros(F, np.int32)
+        vt, vl, vi, vj = (np.zeros((F, max(vis_cap, 1)), np.int32) for _ in range(4))
+        vo = np.zeros((F, max(vis_cap, 1), 12))
+        inv, lid = np.zeros((F, L)), np.zeros((F, L), np.int32)
+        vp = self._vp
+        self._call("viwb_features_window", C.c_int(vis_cap), vp(nlm), vp(nv), vp(vt), vp(vl), vp(vi), vp(vj), vp(vo), vp(inv), vp(lid))
+        tables = [dict(num_landmarks=int(nlm[s]), vis_type=vt[s, : nv[s]].copy(), vis_landmark=vl[s, : nv[s]].copy(), vis_frame_i=vi[s, : nv[s]].copy(),
+                       vis_frame_j=vj[s, : nv[s]].copy(), vis_obs=vo[s, : nv[s]].copy()) for s in range(F)]
+        return tables, [inv[s, : nlm[s]].copy() for s in range(F)], [lid[s, : nlm[s]].copy() for s in range(F)]
+
+    def set_depth(self, inv_depth):
+        """inv_depth: per stream, the landmarks' inverse depths in the last export's numbering"""
+        x = np.zeros((self.F, MAX_LANDMARKS))
+        for s, v in enumerate(inv_depth):
+            v = np.asarray(v, np.float64).reshape(-1)
+            x[s, : len(v)] = v
+        self._call("viwb_features_set_depth", self._vp(x))
+
+    def remove_outliers(self, outliers):
+        """outliers: per stream, per-landmark flags of the last export -> per stream the removed ids, ascending"""
+        x = np.zeros((self.F, MAX_LANDMARKS), np.uint8)
+        for s, v in enumerate(outliers):
+            v = np.asarray(v, np.uint8).reshape(-1)
+            x[s, : len(v)] = v
+        n, ids = np.zeros(self.F, np.int32), np.zeros((self.F, self.M), np.int32)
+        self._call("viwb_features_remove_outliers", self._vp(x), self._vp(n), self._vp(ids))
+        return [ids[s, : n[s]].copy() for s in range(self.F)]
+
+    def predict(self, states, frame_count):
+        """-> per stream None (frame_count < 2: no setPrediction) or (ids, pts_cam [k, 3]), the form Tracker.feedback takes"""
+        st = np.ascontiguousarray(states, np.float64).reshape(self.F, abi.STATE_FIXED)
+        fc = self._per_stream(frame_count, np.int32)
+        n, ids, pts, hp = np.zeros(self.F, np.int32), np.zeros(self.F * self.M, np.int32), np.zeros((self.F * self.M, 3)), np.zeros(self.F, np.uint8)
+        vp = self._vp
+        self._call("viwb_features_predict", vp(st), vp(fc), vp(n), vp(ids), vp(pts), vp(hp))
+        out, o = [], 0
+        for s in range(self.F):
+            out.append((ids[o: o + n[s]].copy(), pts[o: o + n[s]].copy()) if hp[s] else None)
+            o += n[s]
+        return out
+
+    def slide(self, frame_count, shift_depth, marg_R=None, marg_P=None, new_R=None, new_P=None):
+        fc, sh = self._per_stream(frame_count, np.int32), self._per_stream(shift_depth, np.uint8)
+        m = [None if a is None else np.ascontiguousarray(a, np.float64) for a in (marg_R, marg_P, new_R, new_P)]
+        vp = self._vp
+        self._call("viwb_features_slide", vp(fc), vp(sh), vp(m[0]), vp(m[1]), vp(m[2]), vp(m[3]))
+
+    def remove_failures(self):
+        self._call("viwb_features_remove_failures")
+
+    def download(self):
+        """-> per stream dict: ids, start_frame, num_obs, depth, solve_flag [n]; obs [n][11][12] float32; cur_td [n][11]; is_stereo [n][11]"""
+        F, M = self.F, self.M
+        n = np.zeros(F, np.int32)
+        ids, sf, no, fl = (np.zeros((F, M), np.int32) for _ in range(4))
+        dep = np.zeros((F, M))
+        obs, td, ster = np.zeros((F, M, 11, 12), np.float32), np.zeros((F, M, 11)), np.zeros((F, M, 11), np.uint8)
+        vp = self._vp
+        self._call("viwb_features_download", vp(n), vp(ids), vp(sf), vp(no), vp(dep), vp(fl), vp(obs), vp(td), vp(ster))
+        return [dict(ids=ids[s, : n[s]].copy(), start_frame=sf[s, : n[s]].copy(), num_obs=no[s, : n[s]].copy(), depth=dep[s, : n[s]].copy(),
+                     solve_flag=fl[s, : n[s]].copy(), obs=obs[s, : n[s]].copy(), cur_td=td[s, : n[s]].copy(), is_stereo=ster[s, : n[s]].copy()) for s in range(F)]
+
+    def close(self):
+        if self.hnd:
+            self.ctx.lib.viwb_features_destroy(self.hnd)
             self.hnd = C.c_void_p()
 
 
