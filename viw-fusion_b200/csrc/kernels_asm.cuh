@@ -6,13 +6,11 @@
 //   COMMON item (chunk)               : all factors                                 -> [E0 E1 td]^T [E0 E1 td] (91), ^T r (13)
 // Lists are cut into chunks of ASM_CHUNK entries; chunk c of every list is "phase" c.  Items of one phase write
 // disjoint blocks of H, so the consumer adds them phase by phase with plain stores (deterministic).
-//   asm_items  : one warp per item, lanes over the item's outputs, records streamed from HBM/L2 (54 doubles per factor)
-//   syrk       : one block per window, T = sum_k gamma_k w_k w_k^T with a shared-memory tile of W and 4x4 register tiles
+//   asm_items  : ASM_SPLIT warps per item, lanes over the item's outputs, records streamed from HBM/L2 (54 doubles per factor)
 //   assemble_into(target) : called by the solve kernel (packed shared-memory triangle) and by the marginalisation
 //                kernel (dense marginalisation layout): prior J^T J, IMU / wheel / plane J^T J factor by factor,
 //                visual partial sums phase by phase.
 #pragma once
-#include <vector>
 #include "layout.cuh"
 #include "factors.cuh"
 #include "kernels_lin.cuh"
@@ -39,19 +37,15 @@ VIWB_HD void sym_unrank(int e, int &p, int &q) {   // e = p(p+1)/2 + q, 0 <= q <
 }
 
 // ------------------------------------------------------------------------------------------------ asm_items
-// grid: ceil(nitems * split / warps_per_block); mode selects the solver or the marginalisation item table.
+// grid: ceil(nitems * ASM_SPLIT / warps_per_block); mode selects the solver or the marginalisation item table.
 enum { ASM_SPLIT = 4 };
-#ifndef ASM_PAIR_U
-#define ASM_PAIR_U 3
-#endif
-template <int SPLIT>
-VIWB_D void asm_items_body(const BatchDev &bd, int bx, int tid, int nt, int mode) {
+VIWB_D void asm_items_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
+    (void)by; (void)smem;
     const int W = nt < 32 ? nt : 32, wpb = nt / W, lane = tid % W;
-    // Items with the common columns have up to 105 outputs: SPLIT warps share such an item (one slice of the outputs each, the
+    // Items with the common columns have up to 105 outputs: ASM_SPLIT warps share such an item (one slice of the outputs each, the
     // same list walk) instead of one warp walking the list four times.
     const int nitems = (mode == MODE_SOLVE) ? bd.nitems_solve : bd.nitems_marg;
-    const int split = SPLIT;
-    const int wi = bx * wpb + tid / W, it = wi / split, part = wi - it * split;
+    const int wi = bx * wpb + tid / W, it = wi / ASM_SPLIT, part = wi - it * ASM_SPLIT;
     if (it >= nitems) return;
     const int gi = (mode == MODE_SOLVE) ? it : bd.nitems_solve + it;
     const AsmItem item = bd.items[gi];
@@ -59,49 +53,12 @@ VIWB_D void asm_items_body(const BatchDev &bd, int bx, int tid, int nt, int mode
     double *out = bd.asm_out + (size_t)gi * ASM_STRIDE;
     const WinMeta &wm = bd.meta[item.win];
     const int *list = bd.asm_list + (mode == MODE_SOLVE ? wm.list_off : wm.mlist_off);
-    const int rs = rec_stride(bd, mode);
-    const double *recs = bd.vis_rec + (size_t)wm.vis_off * rs;
+    const double *recs = bd.vis_rec + (size_t)wm.vis_off * VREC;
     // outputs of this item; without common columns a FRAME item has only F^T F (21) and F^T r (6 -> stored at 99..104)
     int nout;
     if (item.kind == ITEM_FRAME) nout = item.has_common ? 105 : 27; else if (item.kind == ITEM_PAIR) nout = 36; else nout = 104;
     if (item.kind == ITEM_FRAME && !item.has_common && part == 0) for (int o = 21 + lane; o < 99; o += W) out[o] = 0.0;
-#ifndef ASM_NO_PAIR_TILES
-    if (item.kind == ITEM_PAIR && split == 1) {
-        // F_a^T F_b has 36 outputs: one output per lane needs a second list walk for the last four.  18 lanes with two neighbouring
-        // outputs each (6 loads per entry instead of 4, the F_a column shared) cover the block in ONE walk.
-        enum { PU = ASM_PAIR_U };                                     // list entries in flight per lane (6 loads each)
-        for (int t = lane; t < 18; t += W) {
-            const int pa = t / 3, pb = 2 * (t - 3 * pa);
-            double acc0 = 0.0, acc1 = 0.0;
-            int e = item.lo;
-            int nx[PU];
-            for (int u = 0; u < PU; u++) nx[u] = 0;
-            if (e + PU <= item.hi) for (int u = 0; u < PU; u++) nx[u] = list[e + u];
-            for (; e + PU <= item.hi; e += PU) {
-                int en[PU]; double va[PU], wa[PU], vb0[PU], wb0[PU], vb1[PU], wb1[PU];
-                for (int u = 0; u < PU; u++) en[u] = nx[u];
-                if (e + 2 * PU <= item.hi) for (int u = 0; u < PU; u++) nx[u] = list[e + PU + u];
-                for (int u = 0; u < PU; u++) {
-                    const int role = en[u] & 1;
-                    const double *rc = recs + (size_t)(en[u] >> 1) * rs;
-                    const int ia = (role ? REC_B : REC_A) + pa, ib = (role ? REC_A : REC_B) + pb;
-                    va[u] = rc[ia]; wa[u] = rc[ia + 6]; vb0[u] = rc[ib]; wb0[u] = rc[ib + 6]; vb1[u] = rc[ib + 1]; wb1[u] = rc[ib + 7];
-                }
-                for (int u = 0; u < PU; u++) { acc0 += va[u] * vb0[u] + wa[u] * wb0[u]; acc1 += va[u] * vb1[u] + wa[u] * wb1[u]; }
-            }
-            for (; e < item.hi; e++) {
-                const int ent = list[e], role = ent & 1;
-                const double *rec = recs + (size_t)(ent >> 1) * rs;
-                const int ia = (role ? REC_B : REC_A) + pa, ib = (role ? REC_A : REC_B) + pb;
-                acc0 += rec[ia] * rec[ib] + rec[ia + 6] * rec[ib + 6];
-                acc1 += rec[ia] * rec[ib + 1] + rec[ia + 6] * rec[ib + 7];
-            }
-            out[6 * pa + pb] = acc0; out[6 * pa + pb + 1] = acc1;
-        }
-        return;
-    }
-#endif
-    for (int o0 = lane + W * part; o0 < nout; o0 += W * split) {
+    for (int o0 = lane + W * part; o0 < nout; o0 += W * ASM_SPLIT) {
         int o = o0;
         if (item.kind == ITEM_FRAME && !item.has_common && o0 >= 21) o = 99 + (o0 - 21);
         // operand kinds: 0 = frame slot of a, 1 = frame slot of b (PAIR), 2 = common column, 3 = residual
@@ -125,7 +82,7 @@ VIWB_D void asm_items_body(const BatchDev &bd, int bx, int tid, int nt, int mode
             if (e + 8 <= item.hi) for (int u = 0; u < 4; u++) nx[u] = list[e + 4 + u];
             for (int u = 0; u < 4; u++) {
                 const int role = en[u] & 1;
-                rc[u] = recs + (size_t)(en[u] >> 1) * rs;
+                rc[u] = recs + (size_t)(en[u] >> 1) * VREC;
                 const int ia = (ka == 0) ? (role ? REC_B : REC_A) + ia_c : ia_c;
                 const int ib = (kb == 0) ? (role ? REC_B : REC_A) + ib_c : (kb == 1 ? (role ? REC_A : REC_B) + ib_c : ib_c);
                 va[u] = rc[u][ia]; wa[u] = rc[u][ia + sa]; vb[u] = rc[u][ib]; wb[u] = rc[u][ib + sb];
@@ -134,122 +91,12 @@ VIWB_D void asm_items_body(const BatchDev &bd, int bx, int tid, int nt, int mode
         }
         for (; e < item.hi; e++) {
             const int ent = list[e], role = ent & 1;
-            const double *rec = recs + (size_t)(ent >> 1) * rs;
+            const double *rec = recs + (size_t)(ent >> 1) * VREC;
             const int ia = (ka == 0) ? (role ? REC_B : REC_A) + ia_c : ia_c;
             const int ib = (kb == 0) ? (role ? REC_B : REC_A) + ib_c : (kb == 1 ? (role ? REC_A : REC_B) + ib_c : ib_c);
             acc += rec[ia] * rec[ib] + rec[ia + sa] * rec[ib + sb];
         }
         out[o] = acc;
-    }
-}
-
-VIWB_D void asm_items_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) { (void)by; (void)smem; asm_items_body<1>(bd, bx, tid, nt, mode); }
-VIWB_D void asm_items_split_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) { (void)by; (void)smem; asm_items_body<ASM_SPLIT>(bd, bx, tid, nt, mode); }
-
-// ------------------------------------------------------------------------------------------------ syrk
-// T = sum_k g_k w_k w_k^T (80 x 80, symmetric, both triangles written), tvec = sum_k g_k w_k gl_k.
-// solver: g_k = gamma_k; marginalisation: g_k = 1 / a_k for the landmarks hosted in frame 0 (gamma holds a_k, 0 = skip).
-enum { SYRK_KC = 32 };
-VIWB_HD size_t syrk_smem_doubles() { return (size_t)2 * SYRK_KC * VSUB + 4 * SYRK_KC; }
-// 16-byte asynchronous global -> shared copy (cp.async), commit / wait by groups
-VIWB_D void async_copy16(double *smem_dst, const double *gsrc) {
-#ifdef VIWB_HOST_EMU
-    smem_dst[0] = gsrc[0]; smem_dst[1] = gsrc[1];
-#else
-    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gsrc) : "memory");
-#endif
-}
-VIWB_D void async_commit() {
-#ifndef VIWB_HOST_EMU
-    asm volatile("cp.async.commit_group;\n" ::: "memory");
-#endif
-}
-template <int PENDING> VIWB_D void async_wait() {
-#ifndef VIWB_HOST_EMU
-    asm volatile("cp.async.wait_group %0;\n" ::"n"(PENDING) : "memory");
-#endif
-}
-// Chunks of 32 landmarks stream through two shared-memory buffers: the copy of chunk c+1 is in flight while chunk c is
-// multiplied (4x4 register tiles of the lower triangle, 210 tiles + 20 work items for tvec).
-VIWB_D void syrk_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
-    (void)by;
-    const int w = bx;
-    const WinMeta &m = bd.meta[w];
-    if (mode == MODE_SOLVE && bd.work[w].status != ST_RUNNING) return;
-    if (mode == MODE_MARG && m.margin_flag != 0) return;
-    double *Wb[2] = {smem, smem + SYRK_KC * VSUB};
-    double *gkb[2] = {smem + 2 * SYRK_KC * VSUB, smem + 2 * SYRK_KC * VSUB + SYRK_KC};              // g_k
-    double *ggb[2] = {smem + 2 * SYRK_KC * VSUB + 2 * SYRK_KC, smem + 2 * SYRK_KC * VSUB + 3 * SYRK_KC};  // g_k * gl_k
-    const double *W = bd.lm_W + (size_t)m.lm_off * VSUB, *gam = bd.lm_gamma + m.lm_off, *gl = bd.lm_g + m.lm_off;
-    double *T = bd.Tvis + (size_t)w * VSUB * VSUB, *tv = bd.tvec + (size_t)w * VSUB;
-    const int NT4 = VSUB / 4, ntiles = NT4 * (NT4 + 1) / 2;
-    const int t = tid;
-    const bool live = t < ntiles + NT4, is_vec = t >= ntiles;       // one round: 230 work items <= block size (256); emulation loops below
-    auto stage = [&](int c, int p) {
-        const int k0 = c * SYRK_KC, kc = (m.nlm - k0) < SYRK_KC ? (m.nlm - k0) : SYRK_KC;
-        for (int e = tid; e < kc * VSUB / 2; e += nt) { if (gam[k0 + (2 * e) / VSUB] > 0.0) async_copy16(Wb[p] + 2 * e, W + (size_t)k0 * VSUB + 2 * e); else { Wb[p][2 * e] = 0.0; Wb[p][2 * e + 1] = 0.0; } }
-        async_commit();
-        for (int k = tid; k < kc; k += nt) {
-            double g = gam[k0 + k];
-            if (mode == MODE_MARG) g = marg_pivot_weight(g);
-            gkb[p][k] = g; ggb[p][k] = g * gl[k0 + k];
-        }
-    };
-    const int nchunk = (m.nlm + SYRK_KC - 1) / SYRK_KC;
-#ifdef VIWB_HOST_EMU
-    const int nwork = ntiles + NT4;
-    std::vector<double> accs((size_t)nwork * 16, 0.0);
-#else
-    double acc[16];
-    for (int i = 0; i < 16; i++) acc[i] = 0.0;
-    int tp = 0, tq = 0;
-    if (live && !is_vec) sym_unrank(t, tp, tq); else if (live) tp = t - ntiles;
-#endif
-    if (nchunk > 0) stage(0, 0);
-    for (int c = 0, p = 0; c < nchunk; c++, p ^= 1) {
-        if (c + 1 < nchunk) { stage(c + 1, p ^ 1); async_wait<1>(); } else async_wait<0>();
-        VIWB_SYNC();
-        const int k0 = c * SYRK_KC, kc = (m.nlm - k0) < SYRK_KC ? (m.nlm - k0) : SYRK_KC;
-        const double *Ws = Wb[p], *gk = gkb[p], *gg = ggb[p];
-#ifdef VIWB_HOST_EMU
-        for (int wi = 0; wi < nwork; wi++) {
-            double *acc = accs.data() + (size_t)wi * 16;
-            int tp = 0, tq = 0;
-            const bool is_vec = wi >= ntiles;
-            if (!is_vec) sym_unrank(wi, tp, tq); else tp = wi - ntiles;
-            (void)live;
-#else
-        if (live) {
-#endif
-            if (!is_vec) {
-                for (int k = 0; k < kc; k++) {
-                    const double *r = Ws + k * VSUB; const double g = gk[k];
-                    const double a0 = g * r[4 * tp], a1 = g * r[4 * tp + 1], a2 = g * r[4 * tp + 2], a3 = g * r[4 * tp + 3];
-                    const double b0 = r[4 * tq], b1 = r[4 * tq + 1], b2 = r[4 * tq + 2], b3 = r[4 * tq + 3];
-                    acc[0] += a0 * b0; acc[1] += a0 * b1; acc[2] += a0 * b2; acc[3] += a0 * b3;
-                    acc[4] += a1 * b0; acc[5] += a1 * b1; acc[6] += a1 * b2; acc[7] += a1 * b3;
-                    acc[8] += a2 * b0; acc[9] += a2 * b1; acc[10] += a2 * b2; acc[11] += a2 * b3;
-                    acc[12] += a3 * b0; acc[13] += a3 * b1; acc[14] += a3 * b2; acc[15] += a3 * b3;
-                }
-            } else {
-                for (int k = 0; k < kc; k++) { const double *r = Ws + k * VSUB; const double g = gg[k]; for (int i = 0; i < 4; i++) acc[i] += r[4 * tp + i] * g; }
-            }
-        }
-        VIWB_SYNC();
-    }
-#ifdef VIWB_HOST_EMU
-    for (int wi = 0; wi < nwork; wi++) {
-        const double *acc = accs.data() + (size_t)wi * 16;
-        int tp = 0, tq = 0;
-        const bool is_vec = wi >= ntiles;
-        if (!is_vec) sym_unrank(wi, tp, tq); else tp = wi - ntiles;
-#else
-    if (live) {
-#endif
-        if (!is_vec) {
-            for (int i = 0; i < 4; i++) for (int j = 0; j < 4; j++) { T[(4 * tp + i) * VSUB + 4 * tq + j] = acc[i * 4 + j]; T[(4 * tq + j) * VSUB + 4 * tp + i] = acc[i * 4 + j]; }
-        } else { for (int i = 0; i < 4; i++) tv[4 * tp + i] = acc[i]; }
     }
 }
 

@@ -5,7 +5,7 @@
 //               (<= LMB_FACTORS factors).  Per tile, thread per factor evaluates residual, Huber, tangent Jacobians (the three projection
 //               factors, factor/projection*Factor.cpp) into a shared-memory tile; the block then
 //                 - reduces the per-landmark quantities straight from the tile: a = |J_l|^2, g_l, the cost, the Schur weight gamma and the
-//                   row W = J_p^T J_l -- the 28-double visual records of lin_vis never exist, lm_reduce does not run, and
+//                   row W = J_p^T J_l -- the per-factor records of lin_vis never exist, lm_reduce does not run, and
 //                 - forms G = sum_f X_f^T X_f of every (host, observer) pair from the tile, X = [A | B | r] (2 x 13; G: A^T A | A^T B | A^T r /
 //                   B^T B | B^T r), per chunk of PAIR_CHUNK records, as a true GEMM on the FP64 tensor pipe (three 8 x 8 accumulator tiles, K = 2
 //                   rows per factor): the X records never leave the SM.
@@ -384,7 +384,7 @@ VIWB_D void lin_vis_lm_wide_block(const BatchDev &bd, int bx, int by, int tid, i
 // ------------------------------------------------------------------------------------------------ asm_pairs_wide
 // One warp per chunk of one frame pair's records: G = sum_f X_f^T X_f on the FP64 tensor pipe.  K index of the product = (factor, residual row): a
 // k-step of 4 = two records; lane l feeds X[k = l%4][column l/4 + 8 t] as the A and the B operand of the tiles in tile row / column t.
-// the product of ONE chunk, written to `out` (global: asm_pairs_wide; shared: pair_win) in accumulator order
+// the product of ONE chunk, written to `out` in accumulator order
 template <bool WIDE>
 VIWB_D void pair_chunk(const BatchDev &bd, const AsmItem &item, double *out, int lane) {
     typedef XL<WIDE> L;
@@ -442,16 +442,16 @@ VIWB_D void asm_pairs_wide_block(const BatchDev &bd, int bx, int by, int tid, in
 // output, fixed order.  Keeps the ~100 dependent L2 reads per entry out of the (latency-bound) consumer kernels.
 VIWB_HD int pair_index(int a, int b) { return a * (2 * NFR - a - 1) / 2 + (b - a - 1); }      // a < b
 template <bool WIDE>
-VIWB_D void pair_reduce_body(const BatchDev &bd, int w, int tid, int nt, int mode, int *ab, const double *outs_in = nullptr, size_t ps_in = 0) {
+VIWB_D void pair_reduce_body(const BatchDev &bd, int w, int tid, int nt, int mode, int *ab) {
     typedef XL<WIDE> L;
     const WinMeta &m = bd.meta[w];
     const bool marg = mode == MODE_MARG;
     double *red = bd.pair_red + (size_t)w * PAIR_RED;
     const AsmItem *items = marg ? bd.mpitems + m.mpitem_off : bd.pitems + m.pitem_off;
     const int npi = marg ? m.nmpitems : m.npitems;
-    // the chunk products: the global array (lin_vis_lm, asm_pairs_wide), or (pair_win) the block's own shared memory
-    const size_t PS = outs_in ? ps_in : (marg ? (size_t)XL<true>::OUT : (size_t)bd.pout_stride);
-    const double *outs = outs_in ? outs_in : (marg ? bd.mpair_out + (size_t)m.mpitem_off * PS : bd.pair_out + (size_t)m.pitem_off * PS);
+    // the chunk products of lin_vis_lm / asm_pairs_wide
+    const size_t PS = marg ? (size_t)XL<true>::OUT : (size_t)bd.pout_stride;
+    const double *outs = marg ? bd.mpair_out + (size_t)m.mpitem_off * PS : bd.pair_out + (size_t)m.pitem_off * PS;
     // the items' frame pair and chunk phase, staged once: every output below walks the whole list (a | b << 4 | phase << 8)
     for (int ii = tid; ii < npi; ii += nt) { const AsmItem &it = items[ii]; ab[ii] = it.a | (it.b << 4) | (it.phase << 8); }
     VIWB_SYNC();
@@ -496,40 +496,33 @@ VIWB_D void pair_reduce_block(const BatchDev &bd, int bx, int by, int tid, int n
     if (m.has_common) pair_reduce_body<true>(bd, bx, tid, nt, mode, ab); else pair_reduce_body<false>(bd, bx, tid, nt, mode, ab);
 }
 
-// ------------------------------------------------------------------------------------------------ pair_win
-// asm_pairs_wide + pair_reduce in one kernel (wide records only: compact windows form their chunks in lin_vis_lm, and a batch that holds them does not use it), one block per window: the window's chunk products stay in shared memory (compact: 1.5 KB per chunk, wide: 5 KB)
-// instead of a 0.6 MB round trip through HBM per window and iteration; warps take the chunks round robin, then the block folds them exactly as
-// pair_reduce does.  Opt-in (VIWB_PAIR_WIN=1, and only when the largest window's chunks fit: bd.pwin_smem): with 109 KB of products per block for the
-// bench window only two blocks share an SM and the kernel measured slower than the two-kernel path it would replace (0.66 vs 0.35 ms, r02zd).
-VIWB_HD size_t pair_win_smem_bytes(int chunks, int out_doubles) { return (size_t)chunks * out_doubles * 8 + (size_t)((chunks + 1) & ~1) * 4; }
-template <bool WIDE>
-VIWB_D void pair_win_body(const BatchDev &bd, int w, int tid, int nt, double *smem, int mode) {
-    typedef XL<WIDE> L;
-    const WinMeta &m = bd.meta[w];
-    const bool marg = mode == MODE_MARG;
-    const AsmItem *items = marg ? bd.mpitems + m.mpitem_off : bd.pitems + m.pitem_off;
-    const int npi = marg ? m.nmpitems : m.npitems;
-    const int Wd = nt < 32 ? nt : 32, nwp = nt / Wd, wid = tid / Wd, lane = tid % Wd;
-    for (int ii = wid; ii < npi; ii += nwp) pair_chunk<WIDE>(bd, items[ii], smem + (size_t)ii * L::OUT, lane);
-    VIWB_SYNC();
-    pair_reduce_body<WIDE>(bd, w, tid, nt, mode, (int *)(smem + (size_t)npi * L::OUT), smem, (size_t)L::OUT);
-}
-VIWB_D void pair_win_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
-    (void)by;
-    const WinMeta &m = bd.meta[bx];
-    if (mode == MODE_MARG) { if (m.mfused) pair_win_body<true>(bd, bx, tid, nt, smem, mode); return; }
-    if (!m.fused || !m.has_common || bd.work[bx].status != ST_RUNNING) return;
-    pair_win_body<true>(bd, bx, tid, nt, smem, mode);
-}
-
 // ------------------------------------------------------------------------------------------------ syrk_mma
 // T = sum_k g_k w_k w_k^T (80 x 80, both triangles written, exactly symmetric), tvec = sum_k g_k gl_k w_k.
 // solver: g_k = gamma_k; marginalisation: g_k = 1 / a_k for the landmarks hosted in frame 0 (gamma holds a_k, 0 = skip; marg_pivot_weight).
 // One [80 x K] x [K x 81] product (column 80 of the right operand = gl): 10 x 11 tiles of 8 x 8, of which the 55 upper-triangular ones
 // and the 10 of the tvec column are computed: five warps, warp v owns tile rows v and 9 - v (13 tiles each).  Chunks of 32 landmarks stream
 // through two shared-memory buffers (cp.async); the row stride 88 makes every operand fetch two conflict-free wavefronts.
-enum { SYRK_LD = 88, SYRK_NT = 160 };
+enum { SYRK_KC = 32, SYRK_LD = 88, SYRK_NT = 160 };
 VIWB_HD size_t syrk_mma_smem_doubles() { return (size_t)2 * SYRK_KC * SYRK_LD + 2 * SYRK_KC; }
+// 16-byte asynchronous global -> shared copy (cp.async), commit / wait by groups
+VIWB_D void async_copy16(double *smem_dst, const double *gsrc) {
+#ifdef VIWB_HOST_EMU
+    smem_dst[0] = gsrc[0]; smem_dst[1] = gsrc[1];
+#else
+    const unsigned d = (unsigned)__cvta_generic_to_shared(smem_dst);
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(d), "l"(gsrc) : "memory");
+#endif
+}
+VIWB_D void async_commit() {
+#ifndef VIWB_HOST_EMU
+    asm volatile("cp.async.commit_group;\n" ::: "memory");
+#endif
+}
+template <int PENDING> VIWB_D void async_wait() {
+#ifndef VIWB_HOST_EMU
+    asm volatile("cp.async.wait_group %0;\n" ::"n"(PENDING) : "memory");
+#endif
+}
 VIWB_D void syrk_mma_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
     (void)by;
     const int w = bx;

@@ -28,8 +28,6 @@ VIWB_HD bool marg_skip(const WinMeta &m, int mode) { return mode == MODE_MARG &&
 // the landmark's own axis to O(|w|^2), so dropping it equals the eigen-cut, while dividing by it would inject w w^T / a in a direction set by rounding.
 VIWB_HD double marg_pivot_weight(double a) { return a > 1e-8 ? 1.0 / a : 0.0; }
 
-VIWB_HD int rec_stride(const BatchDev &bd, int mode) { return mode == MODE_SOLVE ? bd.rec_stride_solve : VREC; }
-
 VIWB_HD const double *eval_state(const BatchDev &bd, int w, int mode) {
     return (mode == MODE_SOLVE ? bd.x_cand : bd.x_cur) + bd.meta[w].state_off;
 }
@@ -77,13 +75,13 @@ VIWB_D void prior_setup_block(const BatchDev &bd, int bx, int by, int tid, int n
 }
 
 // ------------------------------------------------------------------------------------------------ lin_vis
-// One thread per factor.  The records (28 / 54 doubles per factor) are assembled in a shared-memory tile with an odd row stride
+// One thread per factor.  The records (VREC doubles per factor) are assembled in a shared-memory tile with an odd row stride
 // and leave the block as one contiguous, fully coalesced stream (a thread storing its own record directly would touch 32
 // different sectors per store instruction).
-VIWB_HD size_t lin_vis_smem_doubles(int nt, int rs) { return (size_t)nt * (rs | 1) + (nt + 7) / 8; }
+VIWB_HD size_t lin_vis_smem_doubles(int nt) { return (size_t)nt * (VREC | 1) + (nt + 7) / 8; }
 VIWB_D void lin_vis_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
     (void)by;
-    const int rs = rec_stride(bd, mode), ts = rs | 1;
+    const int ts = VREC | 1;
     double *tile = smem;
     unsigned char *act = reinterpret_cast<unsigned char *>(smem + (size_t)nt * ts);
     const int f = bx * nt + tid;
@@ -114,15 +112,13 @@ VIWB_D void lin_vis_block(const BatchDev &bd, int bx, int by, int tid, int nt, d
         rec[0] = o.r[0] * sc; rec[1] = o.r[1] * sc;
         for (int k = 0; k < 12; k++) { rec[REC_A + k] = o.JA[k] * sc; rec[REC_B + k] = o.JB[k] * sc; }
         rec[REC_L] = o.Jl[0] * sc; rec[REC_L + 1] = o.Jl[1] * sc;
-        if (rs == VREC) {
-            for (int k = 0; k < 12; k++) { rec[REC_E0 + k] = o.JE0[k] * sc; rec[REC_E1 + k] = o.JE1[k] * sc; }
-            rec[REC_TD] = o.Jtd[0] * sc; rec[REC_TD + 1] = o.Jtd[1] * sc;
-        }
+        for (int k = 0; k < 12; k++) { rec[REC_E0 + k] = o.JE0[k] * sc; rec[REC_E1 + k] = o.JE1[k] * sc; }
+        rec[REC_TD] = o.Jtd[0] * sc; rec[REC_TD + 1] = o.Jtd[1] * sc;
         bd.vis_cost[f] = half_rho;
     }
     VIWB_SYNC();
-    double *out = bd.vis_rec + (size_t)bx * nt * rs;
-    for (int e = tid; e < nrec * rs; e += nt) { const int r = e / rs, q = e - r * rs; if (act[r]) out[e] = tile[(size_t)r * ts + q]; }
+    double *out = bd.vis_rec + (size_t)bx * nt * VREC;
+    for (int e = tid; e < nrec * VREC; e += nt) { const int r = e / VREC, q = e - r * VREC; if (act[r]) out[e] = tile[(size_t)r * ts + q]; }
 }
 
 // ------------------------------------------------------------------------------------------------ lm_reduce
@@ -141,8 +137,8 @@ VIWB_D double lm_warp_sum(double v) {
 #endif
     return v;
 }
-template <bool WIDE>
-VIWB_D void lm_reduce_body(const BatchDev &bd, int bx, int tid, int nt, int mode) {
+VIWB_D void lm_reduce_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) {
+    (void)by; (void)smem;
     const int gid = bx * nt + tid;
     const int k = gid / LM_ROLES, lane = gid % LM_ROLES;
     if (k >= bd.nlm_total) return;
@@ -162,9 +158,8 @@ VIWB_D void lm_reduce_body(const BatchDev &bd, int bx, int tid, int nt, int mode
         return;
     }
     VIWB_SYNCWARP();
-    const int rs = WIDE ? (int)VREC : (int)VREC_COMPACT;
     const int host = bd.vis_fi[f0];
-    double a = 0.0, g = 0.0, c = 0.0, hacc[6] = {0, 0, 0, 0, 0, 0}, e0[WIDE ? 6 : 1] = {0}, e1[WIDE ? 6 : 1] = {0}, tdv = 0.0;
+    double a = 0.0, g = 0.0, c = 0.0, hacc[6] = {0, 0, 0, 0, 0, 0}, e0[6] = {0}, e1[6] = {0}, tdv = 0.0;
     for (int fb = f0; fb < f1; fb += LM_W) {
         const int f = fb + lane;
         const bool on = f < f1;
@@ -172,7 +167,7 @@ VIWB_D void lm_reduce_body(const BatchDev &bd, int bx, int tid, int nt, int mode
         double bv[6] = {0, 0, 0, 0, 0, 0};
         if (on) {
             const int type = bd.vis_type[f];
-            const double *rec = bd.vis_rec + (size_t)f * rs;
+            const double *rec = bd.vis_rec + (size_t)f * VREC;
             const double u0 = rec[REC_L], u1 = rec[REC_L + 1];
             a += u0 * u0 + u1 * u1; g += u0 * rec[0] + u1 * rec[1]; c += bd.vis_cost[f];
             if (type != 2) {
@@ -180,11 +175,9 @@ VIWB_D void lm_reduce_body(const BatchDev &bd, int bx, int tid, int nt, int mode
                 for (int q = 0; q < 6; q++) bv[q] = rec[REC_B + q] * u0 + rec[REC_B + 6 + q] * u1;
                 fj = bd.vis_fj[f];
             }
-            if (WIDE) {
-                for (int q = 0; q < 6; q++) e0[q] += rec[REC_E0 + q] * u0 + rec[REC_E0 + 6 + q] * u1;
-                tdv += rec[REC_TD] * u0 + rec[REC_TD + 1] * u1;
-                if (type != 0) for (int q = 0; q < 6; q++) e1[q] += rec[REC_E1 + q] * u0 + rec[REC_E1 + 6 + q] * u1;
-            }
+            for (int q = 0; q < 6; q++) e0[q] += rec[REC_E0 + q] * u0 + rec[REC_E0 + 6 + q] * u1;
+            tdv += rec[REC_TD] * u0 + rec[REC_TD + 1] * u1;
+            if (type != 0) for (int q = 0; q < 6; q++) e1[q] += rec[REC_E1 + q] * u0 + rec[REC_E1 + 6 + q] * u1;
         }
         // observing-frame blocks: lanes with the same frame add in lane order
 #ifdef VIWB_HOST_EMU
@@ -203,10 +196,12 @@ VIWB_D void lm_reduce_body(const BatchDev &bd, int bx, int tid, int nt, int mode
     }
     a = lm_warp_sum(a); g = lm_warp_sum(g); c = lm_warp_sum(c);
     for (int q = 0; q < 6; q++) hacc[q] = lm_warp_sum(hacc[q]);
-    if (WIDE) { for (int q = 0; q < 6; q++) { e0[q] = lm_warp_sum(e0[q]); e1[q] = lm_warp_sum(e1[q]); } tdv = lm_warp_sum(tdv); }
+    for (int q = 0; q < 6; q++) { e0[q] = lm_warp_sum(e0[q]); e1[q] = lm_warp_sum(e1[q]); }
+    tdv = lm_warp_sum(tdv);
     if (lane != 0) return;
     for (int q = 0; q < 6; q++) W[6 * host + q] += hacc[q];
-    if (WIDE) { for (int q = 0; q < 6; q++) { W[66 + q] = e0[q]; W[72 + q] = e1[q]; } W[78] = tdv; }
+    for (int q = 0; q < 6; q++) { W[66 + q] = e0[q]; W[72 + q] = e1[q]; }
+    W[78] = tdv;
     bd.lm_a[k] = a; bd.lm_g[k] = g; bd.lm_cost[k] = c;
     if (mode == MODE_MARG) { bd.lm_gamma[k] = a; return; }     // marginalisation keeps the pivot itself
     // Jacobi scale (first linearisation only) and the Schur weight for the mu this linearisation will be solved with:
@@ -217,10 +212,6 @@ VIWB_D void lm_reduce_body(const BatchDev &bd, int bx, int tid, int nt, int mode
     double d2 = s; if (d2 < bd.opt.min_lm_diagonal) d2 = bd.opt.min_lm_diagonal; if (d2 > bd.opt.max_lm_diagonal) d2 = bd.opt.max_lm_diagonal;
     bd.lm_gamma[k] = sc * sc / (s + ww.mu_lin * d2);
 }
-
-// two kernels so that the compact-record case is not charged the registers of the wide one (the host picks by rec_stride)
-VIWB_D void lm_reduce_wide_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) { (void)by; (void)smem; lm_reduce_body<true>(bd, bx, tid, nt, mode); }
-VIWB_D void lm_reduce_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) { (void)by; (void)smem; lm_reduce_body<false>(bd, bx, tid, nt, mode); }
 
 // ------------------------------------------------------------------------------------------------ lin_small
 // prior residual: r = r_lin + J_lin dx (marginalization_factor.cpp:361-380); dx in the prior's own column layout

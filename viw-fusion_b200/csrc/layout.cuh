@@ -3,12 +3,12 @@
 // HBM layout (all FP64 unless noted; B windows, concatenated):
 //   x_cur / x_cand      [sum(207 + nlm)]        parameter blocks, fixed-state layout of include/viwb.h + inverse depths
 //   vis_*               visual factor table, sorted by landmark; vis_obs stays [nvis][12] as given
-//   vis_rec             [nvis_total][28 or 54]  per-factor record written by lin_vis: r(2) A(12) B(12) Jl(2) | Jtd(2) E0(12) E1(12); like vis_cost
+//   vis_rec             [nvis_total][54]        per-factor record written by lin_vis: r(2) A(12) B(12) Jl(2) Jtd(2) E0(12) E1(12); like vis_cost
 //                       only allocated when some window's solve or marginalisation takes the unfused path
 //   lm_*                per landmark: a = |J_l|^2, gl = J_l^T r, gamma = c^2/h (Schur weight), W [80] = J_p^T J_l over the
 //                       "visual subspace" (11 poses x 6 | ex0 6 | ex1 6 | td 1 | pad)
 //   imu_rec / wheel_rec / plane_rec   whitened residual + tangent Jacobian of the small factors
-//   Hpp [B][192*192], gfix [B][192]   normal equations over the fixed tangent layout (assembled by gather, no atomics)
+//   Hpk [B][192*193/2], gpk [B][192]  the active normal equations in the solve kernel's skyline order (assembled by gather, no atomics)
 //   Tvis [B][80*80], tvec [B][80]     Schur sums  sum_k gamma_k w_k w_k^T  and  sum_k gamma_k w_k gl_k
 //   per-window solver vectors (scale, D, scaled gradient, Gauss-Newton step) of length 192 + nlm
 #pragma once
@@ -19,9 +19,8 @@ namespace viwb {
 
 enum { NB = 32, NFR = 11, TFIX = 192, SFIX = 207, VSUB = 80, VREC = 54, IMU_REC = 15 + 15 * 30, WHEEL_REC = 6 + 6 * 22,
        PLANE_REC = 3 + 3 * 16, MAXPRI = 200 };
-// record layout: the first VREC_COMPACT doubles (r, A, B, J_lambda) are all a solve needs when ex0/ex1/td are constant;
-// td / E0 / E1 follow and are only written (and the stride only widened to VREC) when some window needs them
-enum { REC_R = 0, REC_A = 2, REC_B = 14, REC_L = 26, REC_TD = 28, REC_E0 = 30, REC_E1 = 42, VREC_COMPACT = 28 };
+// record layout of lin_vis (VREC doubles per factor)
+enum { REC_R = 0, REC_A = 2, REC_B = 14, REC_L = 26, REC_TD = 28, REC_E0 = 30, REC_E1 = 42 };
 enum { BLK_SB0 = 11, BLK_EX0 = 22, BLK_EX1 = 23, BLK_EXW = 24, BLK_PR = 25, BLK_PZ = 26, BLK_SX = 27, BLK_SY = 28, BLK_SW = 29,
        BLK_TD = 30, BLK_TDW = 31 };
 
@@ -62,10 +61,9 @@ struct WinMeta {        // read-only during a solve
     int prior_idx;      // -1: none
     int frame_count;
     int nf;             // active fixed tangent columns (compact)
-    int namb;
     int margin_flag;
-    int item_off, nitems, nphases, list_off;     // assembly items of the solver linearisation (kernels_asm.cuh); list entries are window-local
-    int mitem_off, nmitems, nmphases, mlist_off; // assembly items of the marginalisation linearisation (factors hosted in frame 0)
+    int item_off, nitems, list_off;     // assembly items of the solver linearisation (kernels_asm.cuh); list entries are window-local
+    int mitem_off, nmitems, mlist_off; // assembly items of the marginalisation linearisation (factors hosted in frame 0)
     int has_common;                     // any of ex0 / ex1 / td is an active column (solver); marginalisation always counts them
     int xrec_off, nxrec;                // fused path (wide solver windows): the window's record region in xrec (offset in DOUBLES), number of records
     int pitem_off, npitems;             // fused path: pair items (chunks of one frame pair's records), head item of a pair has phase 0
@@ -107,11 +105,9 @@ struct BatchDev {       // passed by value to every kernel
     int B, nvis_total, nlm_total, nimu_total, nwheel_total, nplane_total, nprior, nitems_solve, nitems_marg;
     int env_max;            // largest esize over the batch (sizes the solve kernel's shared memory)
     int marg_nmax;          // largest prior dimension any window of the batch produces (sizes the eigen-solver's shared memory)
-    int rec_stride_solve;   // VREC_COMPACT if no window of the batch has ex0/ex1/td active, else VREC (marginalisation always uses VREC)
     int n_unfused;          // windows whose solver linearisation runs lin_vis + lm_reduce + asm_items (the others: lin_vis_lm(_wide), WinMeta.fused)
     int n_fused_wide, n_fused_compact, n_munfused, n_mfused;      // fused solver windows by record width; marginalising windows by path
     int nlmb_total, npitems_total, nmpitems_total, pitems_max;
-    int pwin_smem, pwin_smem_marg;      // dynamic shared memory of pair_win (solver / marginalisation mode); 0: a window's chunks do not fit (or, solver, compact windows form theirs in lin_vis_lm), asm_pairs_wide + pair_reduce run instead
     int pout_stride;        // doubles per solver pair item in pair_out: 192 (all fused windows compact) or 640
     const int *mvis_pos;            // [nvis_total] marginalisation: window-local record slot of the factors hosted in frame 0 (-1 otherwise)
     const struct AsmItem *mpitems;  // [nmpitems_total]
@@ -162,7 +158,7 @@ struct BatchDev {       // passed by value to every kernel
     const double *prior_J, *prior_r, *prior_x0;
     double *prior_A, *prior_res, *prior_g;
     // normal equations
-    double *Hpk, *gpk, *gfix, *Tvis, *tvec;   // Hpk [B][TFIX*(TFIX+1)/2] packed active H, gpk [B][TFIX] compact gradient
+    double *Hpk, *gpk, *Tvis, *tvec;   // Hpk [B][TFIX*(TFIX+1)/2] packed active H, gpk [B][TFIX] compact gradient
     // solver vectors, per window at work_off = state_off - 15*w ... stored at vec_off = w*TFIX + lm_off
     double *v_scale, *v_D, *v_sgrad, *v_gn;
     double *v_wug, *v_wun;              // [nlm_total] per landmark w_k . u_g and w_k . (C y) of the current linearisation (solve)

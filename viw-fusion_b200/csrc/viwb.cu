@@ -92,21 +92,12 @@ DEF_KERNEL(vis_expand, 128)
 DEF_KERNEL(setup, 128)
 DEF_KERNEL(prior_setup, 256)
 DEF_KERNEL2(lin_vis, 128, LIN_VIS_MINB)
-#ifndef LM_MINB
-#define LM_MINB 8
-#endif
-DEF_KERNEL2(lm_reduce, 128, LM_MINB)
-DEF_KERNEL(lm_reduce_wide, 128)
+DEF_KERNEL(lm_reduce, 128)
 #ifndef LSM_MINB
 #define LSM_MINB 4      // 128 registers, 4 blocks / SM: the spills of the IMU evaluation (10 threads of the block) cost less than the idle SM (r02n: 0.38 -> 0.25 ms per launch)
 #endif
 DEF_KERNEL2(lin_small, 128, LSM_MINB)
 DEF_KERNEL(asm_items, 128)
-DEF_KERNEL(asm_items_split, 128)
-#ifndef SYRK_MINB
-#define SYRK_MINB 4
-#endif
-DEF_KERNEL2(syrk, 256, SYRK_MINB)
 #ifndef SOLVE_NT
 #define SOLVE_NT 384
 #endif
@@ -121,7 +112,6 @@ DEF_KERNEL(asm_pairs_wide, 128)
 #define PAIR_RED_NT 256
 #endif
 DEF_KERNEL(pair_reduce, PAIR_RED_NT)
-DEF_KERNEL2(pair_win, 256, 2)
 DEF_KERNEL2(syrk_mma, SYRK_NT, 4)
 DEF_KERNEL(reanchor, 32)
 DEF_KERNEL2(marg_prep, 256, 2)
@@ -145,8 +135,6 @@ static void arena_release(Arena &a) { if (a.dev) dev_free(a.dev); if (a.host) ho
 static double now_ms() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
 static bool g_timing = getenv("VIWB_TIMING") != nullptr;
 static bool g_marg_one_kernel = getenv("VIWB_MARG_ONE_KERNEL") != nullptr;      // measurement aid: tred2 + tql2 in one block-per-window kernel (marg_eig)
-static bool g_no_pair_win = getenv("VIWB_PAIR_WIN") == nullptr;      // pair_win (chunk products in shared memory, one block per window) is opt-in: at the bench window's 109 KB per block it measured 0.66 ms against 0.21 + 0.14 for asm_pairs + pair_reduce (profiles/r02zd_probe.txt)
-static bool g_syrk_dfma = getenv("VIWB_SYRK_DFMA") != nullptr;      // measurement aid: the 4x4 register-tiled DFMA SYRK instead of the DMMA one (profiles/: both builds of the Schur GEMM)
 struct viwb_context {
     int device;
     stream_t stream;        // the stream all work of this context is issued on (own_stream unless viwb_set_stream gave another)
@@ -196,7 +184,6 @@ struct viwb_batch {
     bool any_marg;
     int max_iter;
     double max_time;       // max_solver_time_in_seconds (0 = off): checked on the host between rounds, like Ceres' wall-clock test
-    size_t nrec_imu, nrec_wheel, nrec_plane;
 };
 
 static size_t align_up(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -336,16 +323,16 @@ static void lower_count(const viwb_problem &p, int mf, bool allow_fused, WinMeta
     // Column order = elimination order of the dense Cholesky.  The speed-bias blocks come first, newest frame first: each couples
     // only with its neighbour in the IMU chain and two poses, so the factor keeps a narrow profile there (a "skyline": row i is
     // stored from its first structurally non-zero column efirst[i]; Cholesky never fills outside that envelope).
-    int col = 0, amb = 0;
+    int col = 0;
     bool active[NB];
     for (int k = 0; k < NB; k++) {
         m.flags[k] = p.block_flags[k] & 3u; m.mask[k] = p.subset_mask[k];
         active[k] = (p.block_flags[k] & VIWB_BLOCK_PRESENT) && !(p.block_flags[k] & VIWB_BLOCK_CONSTANT) && ref[k];
         m.tcol[k] = -1;
     }
-    for (int f = VIWB_WINDOW_SIZE; f >= 0; f--) { const int k = BLK_SB0 + f; if (active[k]) { m.tcol[k] = (short)col; col += blk_tsize(k); amb += blk_size(k); } }
-    for (int k = 0; k < NB; k++) if (active[k] && m.tcol[k] < 0) { m.tcol[k] = (short)col; col += blk_tsize(k); amb += blk_size(k); }
-    m.nf = col; m.namb = amb + p.num_landmarks;
+    for (int f = VIWB_WINDOW_SIZE; f >= 0; f--) { const int k = BLK_SB0 + f; if (active[k]) { m.tcol[k] = (short)col; col += blk_tsize(k); } }
+    for (int k = 0; k < NB; k++) if (active[k] && m.tcol[k] < 0) { m.tcol[k] = (short)col; col += blk_tsize(k); }
+    m.nf = col;
     {   // symbolic envelope: every factor makes the blocks it touches a clique
         int first_blk[NB];
         for (int k = 0; k < NB; k++) first_blk[k] = m.tcol[k];                 // the diagonal block itself
@@ -425,19 +412,19 @@ static void lower_count(const viwb_problem &p, int mf, bool allow_fused, WinMeta
     lo.marg = m.margin_flag != 0 ? MARG_NONE : mfused ? MARG_WIDE : MARG_UNFUSED;
     m.fused = fused; m.mfused = mfused;
     // the sizes of the chosen paths' tables; lower_fill builds them
-    auto list_sizes = [](const int *fc, const int *pc, int ncom, int &nlist, int &nitems, int &nphases) {      // emit_lists: frame lists, pair lists, common list
-        auto add = [&](int n) { nlist += n; nitems += chunk_count(n); nphases = std::max(nphases, chunk_count(n)); };
+    auto list_sizes = [](const int *fc, const int *pc, int ncom, int &nlist, int &nitems) {      // emit_lists: frame lists, pair lists, common list
+        auto add = [&](int n) { nlist += n; nitems += chunk_count(n); };
         for (int a = 0; a < NFR; a++) add(fc[a]);
         for (int a = 0; a < NFR * NFR; a++) add(pc[a]);
         add(ncom);
     };
-    if (lo.solve == SOLVE_UNFUSED) list_sizes(fcnt, pcnt, m.has_common ? p.num_vis : 0, lo.nlist_s, m.nitems, m.nphases);
+    if (lo.solve == SOLVE_UNFUSED) list_sizes(fcnt, pcnt, m.has_common ? p.num_vis : 0, lo.nlist_s, m.nitems);
     if (lo.solve == SOLVE_COMPACT) {      // the pairs' products are formed per host run, no record is stored
         m.npitems = npit;
         host_runs(p.num_vis, p.vis_landmark, p.vis_frame_i, p.num_landmarks, [&](int h, int, int, int, bool fresh) { if (fresh) { if (lo.run_nt[h]++ == 0) lo.nrun++; lo.nrtile++; } });
     }
     if (lo.solve == SOLVE_WIDE) { m.npitems = npit; m.nxrec = nxrec; }
-    if (lo.marg == MARG_UNFUSED) list_sizes(fcnt0, pcnt0, ncommon0, lo.nlist_m, m.nmitems, m.nmphases);
+    if (lo.marg == MARG_UNFUSED) list_sizes(fcnt0, pcnt0, ncommon0, lo.nlist_m, m.nmitems);
     if (lo.marg == MARG_WIDE) { m.nmpitems = nmpit; m.nmxrec = ncommon0; }
     if (lo.solve == SOLVE_WIDE || lo.marg == MARG_WIDE) m.nlmb = nlmb;
 }
@@ -695,24 +682,11 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     }
     bd.nvis_total = (int)nvis; bd.nlm_total = (int)nlm; bd.nimu_total = (int)nimu; bd.nwheel_total = (int)nwheel; bd.nplane_total = (int)nplane; bd.nprior = (int)npri;
     bd.nitems_solve = (int)nit_s; bd.nitems_marg = (int)nit_m;
-    bd.rec_stride_solve = VREC_COMPACT;
     bd.nlmb_total = (int)nlmb; bd.npitems_total = (int)npit; bd.nmpitems_total = (int)nmpit; bd.nrun_total = (int)nrun;
     bd.pitems_max = 1; for (int w = 0; w < B; w++) bd.pitems_max = std::max(bd.pitems_max, std::max(b->meta[w].npitems, b->meta[w].nmpitems));
-    {   // pair_win keeps a window's chunk products in shared memory: possible when the largest window fits next to a second resident block
-        size_t need_s = 0, need_m = 0;
-        for (int w = 0; w < B; w++) {
-            const WinMeta &mw = b->meta[w];
-            if (mw.fused) need_s = std::max(need_s, pair_win_smem_bytes(mw.npitems, mw.has_common ? (int)XL<true>::OUT : (int)XL<false>::OUT));
-            if (mw.mfused) need_m = std::max(need_m, pair_win_smem_bytes(mw.nmpitems, (int)XL<true>::OUT));
-        }
-        const size_t cap = 110 * 1024;
-        bd.pwin_smem = (!g_no_pair_win && bd.n_fused_compact == 0 && need_s > 0 && need_s <= cap) ? (int)need_s : 0;
-        bd.pwin_smem_marg = (!g_no_pair_win && need_m > 0 && need_m <= cap) ? (int)need_m : 0;
-    }
     bd.pout_stride = bd.n_fused_wide ? (int)XL<true>::OUT : (int)XL<false>::OUT;
     bd.marg_nmax = b->prior_nmax;
     bd.env_max = 1; for (int w = 0; w < B; w++) bd.env_max = std::max(bd.env_max, b->meta[w].esize);
-    for (int w = 0; w < B; w++) if (b->meta[w].has_common) bd.rec_stride_solve = VREC;
     b->total_state = nstate;
     // ---- the slab: every array once -- its device field, its element count, and for an input its view in the staging slab (HostArrays).
     // Inputs come first and are uploaded as one block; a work array is never empty.
@@ -742,7 +716,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     WK(&bd.lm_a, nlm); WK(&bd.lm_g, nlm); WK(&bd.lm_gamma, nlm); WK(&bd.lm_scale, nlm); WK(&bd.lm_cost, nlm); WK(&bd.lm_W, nlm * VSUB); WK(&bd.lm_outlier, nlm);
     WK(&bd.imu_S, nimu * 225); WK(&bd.wheel_S, nwheel * 36); WK(&bd.imu_rec, nimu * IMU_REC); WK(&bd.wheel_rec, nwheel * WHEEL_REC); WK(&bd.plane_rec, nplane * PLANE_REC);
     WK(&bd.prior_A, npJ); WK(&bd.prior_res, npr); WK(&bd.prior_g, npr);
-    WK(&bd.Hpk, (size_t)B * (TFIX * (TFIX + 1) / 2)); WK(&bd.gpk, (size_t)B * TFIX); WK(&bd.gfix, (size_t)B * (TFIX + 8));
+    WK(&bd.Hpk, (size_t)B * (TFIX * (TFIX + 1) / 2)); WK(&bd.gpk, (size_t)B * TFIX);
     WK(&bd.asm_out, (nit_s + nit_m) * ASM_STRIDE); WK(&bd.Tvis, (size_t)B * VSUB * VSUB); WK(&bd.tvec, (size_t)B * VSUB);
     WK(&bd.v_scale, nvec); WK(&bd.v_D, nvec); WK(&bd.v_sgrad, nvec); WK(&bd.v_gn, nvec); WK(&bd.v_wug, nlm); WK(&bd.v_wun, nlm);
     // marginalisation outputs / scratch: sized by the largest prior this batch produces, and not at all when no window marginalises
@@ -789,11 +763,10 @@ static int ensure_attrs(viwb_context *ctx) {
 #ifndef VIWB_HOST_EMU
     if (!ctx->attrs_set) {
         CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_NT, TFIX * (TFIX + 1) / 2) * 8)));
-        CK(cudaFuncSetAttribute(lin_vis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_smem_doubles(128, VREC) * 8)));
+        CK(cudaFuncSetAttribute(lin_vis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_smem_doubles(128) * 8)));
         CK(cudaFuncSetAttribute(lin_vis_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_run_smem_doubles() * 8)));
         CK(cudaFuncSetAttribute(lin_vis_lm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_lm_smem_doubles(true) * 8)));
         CK(cudaFuncSetAttribute(syrk_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(syrk_mma_smem_doubles() * 8)));
-        CK(cudaFuncSetAttribute(pair_win_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 110 * 1024));
         CK(cudaFuncSetAttribute(marg_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_prep_smem_doubles(256, 100) * 8)));
         CK(cudaFuncSetAttribute(marg_tri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_eig_smem_doubles(256, 100) * 8)));
         CK(cudaFuncSetAttribute(marg_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_apply_smem_doubles(128, 100) * 8)));
@@ -816,7 +789,7 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
     CK(dev_d2d(bd.x_cur, bd.x_init, xs, st)); CK(dev_d2d(bd.x_cand, bd.x_init, xs, st));
     if (!(what & RUN_REANCHOR) || (what & RUN_SOLVE)) CK(dev_d2d(bd.x_before, bd.x_init, xs, st));
     CK(dev_d2d(bd.work, b->work_init_dev, sizeof(WinWork) * B, st));
-    const int nt_vis = NT(128), nt_lm = NT(128), nt_small = NT(128), nt_asm = NT(128), nt_syrk = NT(256), nt_solve = NT(SOLVE_NT), nt_marg = NT(256);
+    const int nt_vis = NT(128), nt_lm = NT(128), nt_small = NT(128), nt_asm = NT(128), nt_solve = NT(SOLVE_NT), nt_marg = NT(256);
     const int g_vis = (bd.nvis_total + nt_vis - 1) / nt_vis, g_lm = (bd.nlm_total * LM_ROLES + nt_lm - 1) / nt_lm;
     const size_t sm_small = lin_small_smem_doubles(nt_small) * 8, sm_solve = solve_smem_doubles(nt_solve, bd.env_max) * 8, sm_marg = marg_prep_smem_doubles(nt_marg, bd.marg_nmax) * 8, sm_eig = marg_eig_smem_doubles(nt_marg, bd.marg_nmax) * 8;
     // cost_only: the round after the last allowed iteration only decides accept / reject of the pending candidate (every window
@@ -827,32 +800,27 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
     auto lin = [&](int mode, bool cost_only) {
         const bool solve = mode == MODE_SOLVE;
         const bool unfused = solve ? bd.n_unfused > 0 : bd.n_munfused > 0;      // windows outside the fused path (irregular factor tables)
-        const int rs = solve ? bd.rec_stride_solve : (int)VREC;      // the unfused records (VREC: they and the items carry the common columns)
         const int vmode = cost_only ? (int)MODE_COST : mode;
         if (solve && bd.n_fused_compact > 0) { LAUNCH(lin_vis_lm, bd, bd.nrun_total, 1, NT(LMB_FACTORS), lin_vis_run_smem_doubles() * 8, vmode, st); ctx->launches++; }      // + the compact windows' pair chunks
         if (solve ? bd.n_fused_wide > 0 : bd.n_mfused > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, vmode, st); ctx->launches++; }
         if (unfused) {
-            LAUNCH(lin_vis, bd, g_vis, 1, nt_vis, lin_vis_smem_doubles(nt_vis, rs) * 8, mode, st);
-            if (rs == VREC) LAUNCH(lm_reduce_wide, bd, g_lm, 1, nt_lm, 0, mode, st);
-            else LAUNCH(lm_reduce, bd, g_lm, 1, nt_lm, 0, mode, st);
+            LAUNCH(lin_vis, bd, g_vis, 1, nt_vis, lin_vis_smem_doubles(nt_vis) * 8, mode, st);
+            LAUNCH(lm_reduce, bd, g_lm, 1, nt_lm, 0, mode, st);
             ctx->launches += (g_vis > 0) + (g_lm > 0);
         }
         LAUNCH(lin_small, bd, B, 1, nt_small, sm_small, mode, st); ctx->launches++;
         if (cost_only) return;
-        const int nfi = solve ? bd.npitems_total : bd.nmpitems_total, pw = solve ? bd.pwin_smem : bd.pwin_smem_marg, wpb = nt_asm / (nt_asm < 32 ? nt_asm : 32);
-        if (nfi > 0 && pw > 0) { LAUNCH(pair_win, bd, B, 1, NT(256), (size_t)pw, mode, st); ctx->launches++; }
-        else if (nfi > 0) {
+        const int nfi = solve ? bd.npitems_total : bd.nmpitems_total, wpb = nt_asm / (nt_asm < 32 ? nt_asm : 32);
+        if (nfi > 0) {
             if (!solve || bd.n_fused_wide > 0) { LAUNCH(asm_pairs_wide, bd, (nfi + wpb - 1) / wpb, 1, NT(128), 0, mode, st); ctx->launches++; }
             LAUNCH(pair_reduce, bd, B, 1, NT(PAIR_RED_NT), (size_t)bd.pitems_max * sizeof(int), mode, st); ctx->launches++;
         }
         if (unfused) {
             const int ni = solve ? bd.nitems_solve : bd.nitems_marg;
-            if (rs == VREC) LAUNCH(asm_items_split, bd, (ni * ASM_SPLIT + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
-            else LAUNCH(asm_items, bd, (ni + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
+            LAUNCH(asm_items, bd, (ni * ASM_SPLIT + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
             ctx->launches += ni > 0;
         }
-        if (g_syrk_dfma) LAUNCH(syrk, bd, B, 1, nt_syrk, syrk_smem_doubles() * 8, mode, st);
-        else LAUNCH(syrk_mma, bd, B, 1, NT(SYRK_NT), syrk_mma_smem_doubles() * 8, mode, st);
+        LAUNCH(syrk_mma, bd, B, 1, NT(SYRK_NT), syrk_mma_smem_doubles() * 8, mode, st);
         ctx->launches++;
     };
     if (what & (RUN_SOLVE | RUN_MARG | RUN_LIN_ONLY)) {
