@@ -2,7 +2,8 @@
 libviwb_phases.so (make -C viw-fusion_b200/csrc phases), over the bench's C2 batch (33 x 48 = 1584 windows).
 
 Thread 0 of each window's block reads the SM clock at the barrier-delimited phase boundaries; only launches that compute a step are
-counted.  Per phase the table gives the mean cycles per such launch over the batch, the p90 over the windows of each window's own
+counted.  The Cholesky is split per panel into thread 0's warp factoring the diagonal block, the panel solve up to its barrier and the
+trailing update up to the next one; the back-substitution per block into the block solve and the row update up to its barrier.  Per phase the table gives the mean cycles per such launch over the batch, the p90 over the windows of each window's own
 mean per launch, and the mean / p90 over the windows of the cycles summed over a whole solve.  The card's name, power limit and SM
 clocks are read in the same call.
 Usage (GPU): python profiles/solve_phase_probe.py [path/to/libviwb_phases.so] [--runs 3] [--json OUT]"""
@@ -21,8 +22,9 @@ sys.path.insert(0, os.path.join(ROOT, "viw-fusion_b200", "python"))
 import bench  # noqa: E402
 from viwb import abi, lib  # noqa: E402
 
-PHASES = ["prologue + phase A", "assembly", "D + scaling", "Cauchy (symv + landmarks 1)", "Schur subtraction", "Cholesky",
-          "back-substitution", "landmark pass 2", "reload + symv + forms", "dogleg + candidate"]
+PHASES = ["prologue + phase A", "assembly", "D + scaling", "Cauchy (symv + landmarks 1)", "Schur subtraction", "Cholesky: diagonal block",
+          "Cholesky: panel solve", "Cholesky: trailing update", "back-substitution: block solve", "back-substitution: row update",
+          "landmark pass 2", "reload + symv + forms", "dogleg + candidate"]
 
 
 def gpu_info():

@@ -11,6 +11,7 @@
 // windows share an SM.  All quadratic forms are evaluated on the *unscaled* matrices with unscaled directions
 // u = c o (v / D), which equals Ceres' J_scaled products exactly.
 #pragma once
+#include <vector>
 #include "layout.cuh"
 #include "factors.cuh"
 #include "kernels_asm.cuh"
@@ -66,10 +67,8 @@ struct SolveSmem {
     int *rp, *fst;   // row pointers (nf + 1) and first columns (nf)
     double *g, *sc, *D, *sg, *y, *u, *Hu, *ug, *uvis, *red, *bc, *chol, *dinv, *xo, *Pt;
     int *amap, *vmap;
-    unsigned char *tl;   // per Cholesky panel: the count, then the trailing 4-row groups that reach the panel (chol_tile_lists)
 };
-enum { CHOL_TLD = 52 };  // bytes per panel in tl: the count + up to (TFIX + 4) / 4 = 49 groups
-VIWB_HD size_t solve_smem_doubles(int nt, int esize) { return (size_t)((esize + 1) & ~1) + 9 * TFIX + 2 * VSUB + 5 * 32 + 16 + 2 * TFIX + 2 + (size_t)((nt + 31) / 32) * 48 + 2 * TFIX + 8 * (TFIX + 4) + 2 + TFIX / 8 * CHOL_TLD / 8; }   // ints: amap, vmap, rp, fst; bytes: tl
+VIWB_HD size_t solve_smem_doubles(int nt, int esize) { return (size_t)((esize + 1) & ~1) + 9 * TFIX + 2 * VSUB + 5 * 32 + 16 + 2 * TFIX + 2 + (size_t)((nt + 31) / 32) * 48 + 2 * TFIX + 8 * (TFIX + 4) + 2 * TFIX + 2; }   // ints: amap, vmap, rp, fst
 VIWB_D void carve(SolveSmem &s, double *smem, int nt, int esize) {
     double *p = smem;
     s.L = p; p += (size_t)((esize + 1) & ~1);
@@ -82,7 +81,6 @@ VIWB_D void carve(SolveSmem &s, double *smem, int nt, int esize) {
     if ((p - smem) & 1) p++;                    // Pt is read with 16-byte vector loads
     s.Pt = p; p += 8 * (TFIX + 4);
     s.amap = (int *)p; s.vmap = s.amap + TFIX; s.rp = s.vmap + TFIX; s.fst = s.rp + TFIX + 2;
-    s.tl = (unsigned char *)(p + 2 * TFIX + 2);
 }
 // entry (i, j), j <= i, of the skyline; must lie inside the envelope
 #define SKY(s, i, j) ((s).L[(s).rp[i] - (s).fst[i] + (j)])
@@ -152,14 +150,13 @@ VIWB_D double warp_dot80(const double *W, const double *v, int lane) {
 // Blocked (panel width 8) in-place Cholesky of the packed lower triangle with the right-hand side carried as an extra
 // row n, so that on exit y = L^-1 b (forward substitution for free).  Returns false on a non-positive pivot
 // (Eigen LLT semantics: schur_complement_solver.cc -> LINEAR_SOLVER_FAILURE).  2 barriers per panel:
-//   every warp factors the 8x8 diagonal block redundantly (8 lanes, one row each, in registers; pivots through rsqrt so
+//   every warp that holds panel rows factors the 8x8 diagonal block redundantly (8 lanes, one row each, in registers; pivots through rsqrt so
 //   that the panel rows multiply instead of divide) into its own scratch, so no barrier separates it from the panel solve;
 //   one thread per panel row, which also drops its 8 results into a column-major panel buffer Pt[8][rows]; the trailing
 //   update then runs 4x4 register tiles whose operands are 32-byte vector loads from Pt (conflict-free), not strided
 //   reads of the packed triangle.
 // scratch: nwarps * 48 doubles (36 packed block entries + 8 inverse pivots + flag); dinv[n] receives 1 / L_kk;
 // Pt: 8 * CHOL_LDP doubles, 16-byte aligned.
-enum { CHOL_NB = 8, CHOL_SCR = 48, CHOL_LDP = TFIX + 4 };
 VIWB_D void load4(const double *p, double *o) {
 #ifdef VIWB_HOST_EMU
     o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = p[3];
@@ -168,25 +165,69 @@ VIWB_D void load4(const double *p, double *o) {
     o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
 #endif
 }
-// Per panel (trailing rows r0.. = c0 + nb..), the 4-row groups ti (rows r0 + 4 ti ..) holding a row that reaches the panel (first stored
-// column < r0; row n, the right-hand side, always does): the trailing update enumerates only the tiles between two such groups.  The
-// lists depend on the skyline alone and are built once per launch.
-template <typename Fst>
-VIWB_D void chol_tile_lists(const Fst *fst, int n, unsigned char *tl, int tid, int nt) {
-    for (int p = tid; p * CHOL_NB < n; p += nt) {
-        const int c0 = p * CHOL_NB, r0 = c0 + ((n - c0) < CHOL_NB ? (n - c0) : CHOL_NB), mt = (n + 1 - r0 + 3) / 4;
-        unsigned char *lp = tl + p * CHOL_TLD;
-        int na = 0;
-        for (int ti = 0; ti < mt; ti++) {
-            bool hit = false;
-            for (int a = 0; a < 4; a++) { const int i = r0 + 4 * ti + a; if (i <= n && (i == n || fst[i] < r0)) hit = true; }
-            if (hit) lp[1 + na++] = (unsigned char)ti;
+enum { CHOL_NB = 8, CHOL_SCR = 48, CHOL_LDP = TFIX + 4 };
+// Phase probe (measurement build only, `make phases` -> libviwb_phases.so): thread 0 reads clock64() at the barrier-delimited phase
+// boundaries of a launch that computes a step and adds the cycles since the previous boundary to its window's slot of the phase.
+// The sub-phases of the Cholesky and the back-substitution are summed in registers and written once per factorisation (SOLVE_FLUSH).
+// Launches that only decide the pending candidate and stop are not counted.  The product library compiles none of this.
+enum { SPH_PRO, SPH_ASM, SPH_DSC, SPH_CAUCHY, SPH_SCHUR, SPH_CHOL_DIAG, SPH_CHOL_PANEL, SPH_CHOL_TRAIL, SPH_BACK_SOLVE, SPH_BACK_UPD,
+       SPH_LM2, SPH_FORMS, SPH_DOGLEG, SPH_N, SPH_STEPS = SPH_N, SPH_FACT, SPH_SLOTS, SPH_MAXW = 8192,
+       SPH_SUB0 = SPH_CHOL_DIAG, SPH_NSUB = SPH_BACK_UPD + 1 - SPH_CHOL_DIAG };
+#if defined(VIWB_SOLVE_PROBE) && !defined(VIWB_HOST_EMU)
+__device__ unsigned long long g_solve_phase[SPH_MAXW * SPH_SLOTS];
+struct SolveClock { int w; long long t, sub[SPH_NSUB]; };
+#define SOLVE_PROBE_START() SolveClock sph; sph.w = w; sph.t = clock64(); for (int q_ = 0; q_ < SPH_NSUB; q_++) sph.sub[q_] = 0
+#define SOLVE_MARK(p) do { if (tid == 0 && w < SPH_MAXW) { const long long t_ = clock64(); g_solve_phase[w * SPH_SLOTS + (p)] += t_ - sph.t; sph.t = t_; } } while (0)
+#define SOLVE_COUNT(p) do { if (tid == 0 && w < SPH_MAXW) g_solve_phase[w * SPH_SLOTS + (p)]++; } while (0)
+#define SOLVE_LAP(p) do { if (tid == 0) { const long long t_ = clock64(); sph.sub[(p) - SPH_SUB0] += t_ - sph.t; sph.t = t_; } } while (0)
+#define SOLVE_FLUSH() do { if (tid == 0 && sph.w < SPH_MAXW) for (int q_ = 0; q_ < SPH_NSUB; q_++) { g_solve_phase[sph.w * SPH_SLOTS + SPH_SUB0 + q_] += sph.sub[q_]; sph.sub[q_] = 0; } } while (0)
+#else
+struct SolveClock {};
+#define SOLVE_PROBE_START() SolveClock sph; (void)sph
+#define SOLVE_MARK(p) ((void)0)
+#define SOLVE_COUNT(p) ((void)0)
+#define SOLVE_LAP(p) ((void)0)
+#define SOLVE_FLUSH() ((void)0)
+#endif
+
+// The factorisation plan of one envelope, built once by the host lowering (viwb.cu chol_plan_build) and shared by the windows with that
+// envelope: ints  rp[0..n]  (skyline row pointers),  toff[0..np]  (panel p's trailing-update tiles are tiles[toff[p] .. toff[p+1])),  tiles.
+// A tile is the 4x4 block of rows r0 + 4 ti.., columns r0 + 4 tk.. (r0: the panel's first trailing row, tk <= ti) that receives at least one
+// entry; its word is ti | tk << 8 | on << 16, bit 4 a + b of `on` set when entry (r0 + 4 ti + a, r0 + 4 tk + b) receives the panel's update:
+// the row reaches the panel (first stored column < r0; row n, the right-hand side, always does), so does the column (< n), and it lies on or
+// below the diagonal.  Every receiving entry is in exactly one tile.
+VIWB_HD int chol_panels(int n) { return (n + CHOL_NB - 1) / CHOL_NB; }
+VIWB_HD int chol_plan_head(int n) { return n + 1 + chol_panels(n) + 1; }
+inline void chol_plan_build(const short *efirst, int n, std::vector<int> &plan) {
+    const int np = chol_panels(n), head = chol_plan_head(n);
+    plan.assign((size_t)head, 0);
+    for (int i = 0; i < n; i++) plan[i + 1] = plan[i] + i - efirst[i] + 1;
+    std::vector<unsigned> rows, cols;      // per 4-row group of the panel's trailing rows: which rows / columns reach the panel
+    for (int p = 0; p < np; p++) {
+        plan[n + 1 + p] = (int)plan.size() - head;
+        const int r0 = (p + 1) * CHOL_NB < n ? (p + 1) * CHOL_NB : n, mt = (n + 1 - r0 + 3) / 4;
+        rows.assign(mt, 0u); cols.assign(mt, 0u);
+        for (int i = r0; i <= n; i++) {
+            const unsigned bit = 1u << ((i - r0) & 3);
+            if (i == n) rows[(i - r0) >> 2] |= bit;
+            else if (efirst[i] < r0) { rows[(i - r0) >> 2] |= bit; cols[(i - r0) >> 2] |= bit; }
         }
-        lp[0] = (unsigned char)na;
+        for (int ti = 0; ti < mt; ti++)
+            for (int tk = 0; tk <= ti; tk++) {
+                unsigned on = 0;
+                for (int a = 0; a < 4; a++) if ((rows[ti] >> a) & 1u) on |= cols[tk] << (4 * a);
+                if (tk == ti) on &= 0xf731u;          // on or below the diagonal: column b <= row a
+                if (on) plan.push_back((int)((unsigned)ti | (unsigned)tk << 8 | on << 16));
+            }
     }
+    plan[n + 1 + np] = (int)plan.size() - head;
 }
 VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double *y, int n, int tid, int nt, double *scratch, double *dinv, double *Pt,
-                                const unsigned char *tl) {
+                                const int *__restrict__ plan, SolveClock &sph) {
+    (void)sph;
+    const int yoff = (int)(y - L);
+    const int *toff = plan + n + 1;
+    const unsigned *tiles = reinterpret_cast<const unsigned *>(plan + chol_plan_head(n));
     // skyline rows: ROW(i)[j] is entry (i, j) for fst[i] <= j <= i; row n is the right-hand side (dense).  FST(i) = first stored column.
 #define ROW(i) ((i) < n ? L + rp[i] - fst[i] : y)
 #define FST(i) ((i) < n ? fst[i] : 0)
@@ -194,8 +235,13 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
     double *my = scratch + (size_t)(tid >> 5) * CHOL_SCR;      // this warp's copy of the factored diagonal block
     for (int c0 = 0; c0 < n; c0 += CHOL_NB) {
         const int nb = (n - c0) < CHOL_NB ? (n - c0) : CHOL_NB;
+        const int r0 = c0 + nb;
+        const int nr = n + 1 - r0, mt = (nr + 3) / 4;       // panel rows r0..n (row n = rhs), padded to whole 4-row tiles
+        // only the warps that hold panel rows factor the diagonal block (warp 0 always: row n, dinv and the block's write-back); the others
+        // would only take issue slots from them
+        const bool fac = (tid & ~31) < 4 * mt;
 #ifdef VIWB_HOST_EMU
-        {   // single-thread statement of the same arithmetic
+        if (fac) {   // single-thread statement of the same arithmetic
             (void)lane;
             my[44] = 1.0;
             double a[8][8];
@@ -211,7 +257,7 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
             for (int i = 0; i < nb; i++) for (int j = 0; j <= i; j++) my[i * (i + 1) / 2 + j] = a[i][j];
         }
 #else
-        {
+        if (fac) {
             double a[8];
             const bool act = lane < nb;
             const int rr = c0 + (act ? lane : 0), fr = fst[rr];
@@ -240,10 +286,13 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
             __syncwarp();
         }
 #endif
-        if (my[44] == 0.0) return false;                    // every warp reaches the same verdict
-        const int r0 = c0 + nb;
-        const int nr = n + 1 - r0, mt = (nr + 3) / 4;       // panel rows r0..n (row n = rhs), padded to whole 4-row tiles
-        // panel rows: x_k = (a_ik - sum_m x_m L_km) / L_kk; columns left of a row's envelope are (and stay) structural zeros
+        SOLVE_LAP(SPH_CHOL_DIAG);
+        // this panel's tiles; the first word is fetched before the panel solve (the plan does not depend on the matrix)
+        const unsigned *tp = tiles + toff[c0 / CHOL_NB];
+        const int ntp = toff[c0 / CHOL_NB + 1] - toff[c0 / CHOL_NB];
+        unsigned wd = tid < ntp ? tp[tid] : 0u;
+        // panel rows (a failed pivot leaves inverse pivots of 0 here; the verdict is read after the barrier and the factor discarded):
+        // x_k = (a_ik - sum_m x_m L_km) / L_kk; columns left of a row's envelope are (and stay) structural zeros
         for (int i = r0 + tid; i < r0 + 4 * mt; i += nt) {
             double x[8];
 #pragma unroll
@@ -269,21 +318,17 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
         }
         for (int r = tid; r < nb; r += nt) dinv[c0 + r] = my[36 + r];
         VIWB_SYNC();
+        SOLVE_LAP(SPH_CHOL_PANEL);
+        if (scratch[44] == 0.0) return false;               // warp 0's verdict, the same as every factoring warp's: every thread returns here
         // factored diagonal block back into the matrix (only now: the other warps have finished reading the unfactored one)
         for (int r = tid; r < nb; r += nt) { double *rk = ROW(c0 + r) + c0; const int fr = FST(c0 + r); for (int j = 0; j <= r; j++) if (c0 + j >= fr) rk[j] = my[r * (r + 1) / 2 + j]; }
-        // trailing update with 4x4 register tiles over rows i in [r0, n], columns k in [r0, min(i, n-1)]; a tile whose row group or
-        // column group lies entirely right of the panel (first stored column >= r0) has nothing to receive: only the row groups of the
-        // panel's list are paired, and a column group that reaches the panel through row n alone is skipped
-        const unsigned char *lp = tl + (c0 / CHOL_NB) * CHOL_TLD;
-        const int na = lp[0], ntile = na * (na + 1) / 2;
-        for (int t = tid; t < ntile; t += nt) {
-            int ai, ak; sym_unrank(t, ai, ak);
-            const int ti = lp[1 + ai], tk = lp[1 + ak];
+        // trailing update with 4x4 register tiles over the plan's tiles of this panel: each receiving entry a_ik -= sum_m L_im L_km once
+        for (int t = tid; t < ntp; t += nt) {
+            const unsigned cur = wd;
+            if (t + nt < ntp) wd = tp[t + nt];
+            const int ti = (int)(cur & 0xffu), tk = (int)((cur >> 8) & 0xffu);
+            const unsigned on = cur >> 16;
             const int ib = r0 + 4 * ti, kb = r0 + 4 * tk;
-            bool hit_k = false;
-#pragma unroll
-            for (int a = 0; a < 4; a++) if (kb + a < n && FST(kb + a) < r0) hit_k = true;
-            if (!hit_k) continue;
             double acc[16];
 #pragma unroll
             for (int q = 0; q < 16; q++) acc[q] = 0.0;
@@ -296,92 +341,74 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
 #pragma unroll
                     for (int b2 = 0; b2 < 4; b2++) acc[a * 4 + b2] += li[a] * lk[b2];
             }
-#ifndef SOLVE_NO_BATCH_RMW
             // all sixteen current values are fetched before the first store (four different row pointers: the compiler has to assume they alias)
-            {
-                double *rp4[4]; bool rowok[4], colok[4];
+            int ro[4];      // the rows as offsets from L (row n, the right-hand side y, is carved from the same shared block)
 #pragma unroll
-                for (int a = 0; a < 4; a++) { const int i = ib + a; rowok[a] = i <= n && FST(i) < r0; rp4[a] = rowok[a] ? ROW(i) : L; }
+            for (int a = 0; a < 4; a++) ro[a] = ((on >> (4 * a)) & 0xfu) ? (ib + a < n ? rp[ib + a] - fst[ib + a] : yoff) : 0;
 #pragma unroll
-                for (int b2 = 0; b2 < 4; b2++) { const int k = kb + b2; colok[b2] = k < n && FST(k) < r0; }
+            for (int a = 0; a < 4; a++)
 #pragma unroll
-                for (int a = 0; a < 4; a++)
+                for (int b2 = 0; b2 < 4; b2++) acc[a * 4 + b2] = ((on >> (a * 4 + b2)) & 1u) ? L[ro[a] + kb + b2] - acc[a * 4 + b2] : 0.0;
 #pragma unroll
-                    for (int b2 = 0; b2 < 4; b2++) { const bool on = rowok[a] && colok[b2] && kb + b2 <= ib + a; acc[a * 4 + b2] = on ? rp4[a][kb + b2] - acc[a * 4 + b2] : 0.0; }
+            for (int a = 0; a < 4; a++)
 #pragma unroll
-                for (int a = 0; a < 4; a++)
-#pragma unroll
-                    for (int b2 = 0; b2 < 4; b2++) { if (rowok[a] && colok[b2] && kb + b2 <= ib + a) rp4[a][kb + b2] = acc[a * 4 + b2]; }
-            }
-#else
-#pragma unroll
-            for (int a = 0; a < 4; a++) { const int i = ib + a; if (i <= n && FST(i) < r0) { double *ri = ROW(i);
-#pragma unroll
-                for (int b2 = 0; b2 < 4; b2++) { const int k = kb + b2; if (k < n && k <= i && FST(k) < r0) ri[k] -= acc[a * 4 + b2]; } } }
-#endif
+                for (int b2 = 0; b2 < 4; b2++) if ((on >> (a * 4 + b2)) & 1u) L[ro[a] + kb + b2] = acc[a * 4 + b2];
         }
         VIWB_SYNC();
+        SOLVE_LAP(SPH_CHOL_TRAIL);
     }
 #undef ROW
 #undef FST
     return true;
 }
-// back substitution L^T x = y (blocks of 8 from the bottom): every thread solves the 8x8 triangular block redundantly from
-// broadcast reads (no barrier between the block solve and the update), then all threads update the rows above.  One barrier
-// per block.  Result in y; xo is scratch of n doubles.
-VIWB_D void chol_backsolve_blocked(const double *L, const int *rp, const int *fst, double *y, const double *dinv, double *xo, int n, int tid, int nt) {
-    const int nblk = (n + CHOL_NB - 1) / CHOL_NB;
+// back substitution L^T x = y (blocks of 8 from the bottom): every thread that needs it solves the 8x8 triangular block redundantly from
+// broadcast reads (no barrier between the block solve and the update), then the rows above that the block's columns reach (from the
+// block's first stored column on) are updated.  One barrier per block.  Result in y; xo is scratch of n doubles.
+VIWB_D void chol_backsolve_blocked(const double *L, const int *rp, const int *fst, double *y, const double *dinv, double *xo, int n, int tid, int nt,
+                                   SolveClock &sph) {
+    (void)sph;
+    const int nblk = chol_panels(n);
     for (int bi = nblk - 1; bi >= 0; bi--) {
         const int c0 = bi * CHOL_NB, nb = (n - c0) < CHOL_NB ? (n - c0) : CHOL_NB;
         double x[8];
         const double *rw[8]; int fr[8];              // the block's skyline rows and their first columns
 #pragma unroll
         for (int m = 0; m < 8; m++) { const int r = (m < nb) ? c0 + m : c0; rw[m] = L + rp[r] - fst[r]; fr[m] = fst[r]; }
+        int lo = fr[0];
+#pragma unroll
+        for (int k = 1; k < 8; k++) lo = fr[k] < lo ? fr[k] : lo;
+        // only the threads that store the block's solution or update a row above solve the block
+        const bool act = tid < CHOL_NB || lo + tid < c0;
 #pragma unroll
         for (int k = 7; k >= 0; k--) {
             x[k] = 0.0;
-            if (k < nb) {
+            if (act && k < nb) {
                 double v = y[c0 + k];
 #pragma unroll
                 for (int m = 7; m > k; m--) if (m < nb && c0 + k >= fr[m]) v -= rw[m][c0 + k] * x[m];
                 x[k] = v * dinv[c0 + k];
             }
         }
-        if (tid == 0) {
 #pragma unroll
-            for (int k = 0; k < 8; k++) if (k < nb) xo[c0 + k] = x[k];
-        }
-        for (int i = tid; i < c0; i += nt) {
+        for (int k = 0; k < 8; k++) if (k < nb && tid == (k < nt ? k : 0)) xo[c0 + k] = x[k];
+        SOLVE_LAP(SPH_BACK_SOLVE);
+        for (int i = lo + tid; i < c0; i += nt) {
             double v = y[i];
 #pragma unroll
             for (int k = 0; k < 8; k++) if (k < nb && i >= fr[k]) v -= rw[k][i] * x[k];
             y[i] = v;
         }
         VIWB_SYNC();
+        SOLVE_LAP(SPH_BACK_UPD);
     }
     for (int i = tid; i < n; i += nt) y[i] = xo[i];
     VIWB_SYNC();
+    SOLVE_LAP(SPH_BACK_UPD);
 }
 
 VIWB_D void terminate(WinWork &ww, int term) { ww.status = ST_DONE; ww.term = term; }
 
 enum { SCHUR_U = 4 };      // envelope entries per thread and trip of the Schur subtraction
-
-// Phase probe (measurement build only, `make phases` -> libviwb_phases.so): thread 0 reads clock64() at the barrier-delimited phase
-// boundaries of a launch that computes a step and adds the cycles since the previous boundary to its window's slot of the phase.
-// Launches that only decide the pending candidate and stop are not counted.  The product library compiles none of this.
-enum { SPH_PRO, SPH_ASM, SPH_DSC, SPH_CAUCHY, SPH_SCHUR, SPH_CHOL, SPH_BACK, SPH_LM2, SPH_FORMS, SPH_DOGLEG, SPH_N,
-       SPH_STEPS = SPH_N, SPH_FACT, SPH_SLOTS, SPH_MAXW = 8192 };
-#if defined(VIWB_SOLVE_PROBE) && !defined(VIWB_HOST_EMU)
-__device__ unsigned long long g_solve_phase[SPH_MAXW * SPH_SLOTS];
-#define SOLVE_PROBE_START() long long sph_t = clock64()
-#define SOLVE_MARK(p) do { if (tid == 0 && w < SPH_MAXW) { const long long t_ = clock64(); g_solve_phase[w * SPH_SLOTS + (p)] += t_ - sph_t; sph_t = t_; } } while (0)
-#define SOLVE_COUNT(p) do { if (tid == 0 && w < SPH_MAXW) g_solve_phase[w * SPH_SLOTS + (p)]++; } while (0)
-#else
-#define SOLVE_PROBE_START() ((void)0)
-#define SOLVE_MARK(p) ((void)0)
-#define SOLVE_COUNT(p) ((void)0)
-#endif
 
 // max |x - Plus(x, -g)| over one fixed block (ambient infinity norm of the projected gradient step)
 VIWB_D double block_grad_inf(int b, unsigned mask, const double *x, const double *gneg) {
@@ -404,7 +431,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
     SolveSmem s; carve(s, smem, nt, bd.env_max);
     const int nf = m.nf, N = m.nlm, vo = vec_off(bd, w);
     for (int i = tid; i < nf; i += nt) s.fst[i] = m.efirst[i];
-    if (tid == 0) { int acc = 0; for (int i = 0; i < nf; i++) { s.rp[i] = acc; acc += i - m.efirst[i] + 1; } s.rp[nf] = acc; }
+    for (int i = tid; i <= nf; i += nt) s.rp[i] = bd.chol_plan[m.plan_off + i];
     double *x = bd.x_cur + m.state_off, *xc = bd.x_cand + m.state_off;
     double *g_scale = bd.v_scale + vo, *g_D = bd.v_D + vo, *g_sg = bd.v_sgrad + vo, *g_gn = bd.v_gn + vo;
     double *wug = bd.v_wug + m.lm_off, *wun = bd.v_wun + m.lm_off;      // per landmark: w_k . u_g (Cauchy direction) and w_k . (C y) (Gauss-Newton step), reused by the quadratic forms
@@ -420,7 +447,6 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
         s.amap[m.tcol[b] + k] = blk_toff(b) + k;
         s.vmap[m.tcol[b] + k] = blk_voff(b) >= 0 ? blk_voff(b) + k : -1;
     }
-    chol_tile_lists(m.efirst, nf, s.tl, tid, nt);
     VIWB_SYNC();
 
     if (mode == 2) { assemble_H(bd, w, s, nf, Hpk, gpk, tid, nt); return; }     // debug hook: normal equations only
@@ -603,11 +629,10 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 SOLVE_COUNT(SPH_FACT);
                 h_dirty = true;
                 if (tid == 0) ww.num_linear++;
-                bool ok = cholesky_packed_rhs(s.L, s.rp, s.fst, s.y, nf, tid, nt, s.chol, s.dinv, s.Pt, s.tl);
-                SOLVE_MARK(SPH_CHOL);
+                bool ok = cholesky_packed_rhs(s.L, s.rp, s.fst, s.y, nf, tid, nt, s.chol, s.dinv, s.Pt, bd.chol_plan + m.plan_off, sph);
+                if (ok) chol_backsolve_blocked(s.L, s.rp, s.fst, s.y, s.dinv, s.xo, nf, tid, nt, sph);
+                SOLVE_FLUSH();
                 if (ok) {
-                    chol_backsolve_blocked(s.L, s.rp, s.fst, s.y, s.dinv, s.xo, nf, tid, nt);
-                    SOLVE_MARK(SPH_BACK);
                     // back-substitute the inverse depths (scaled): y_k = (c g_k - c w_k . (C y_f)) / h_k
                     for (int i = tid; i < nf; i += nt) s.u[i] = s.sc[i] * s.y[i];
                     VIWB_SYNC();

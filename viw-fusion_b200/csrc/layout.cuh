@@ -9,6 +9,7 @@
 //                       "visual subspace" (11 poses x 6 | ex0 6 | ex1 6 | td 1 | pad)
 //   imu_rec / wheel_rec / plane_rec   whitened residual + tangent Jacobian of the small factors
 //   Hpk [B][192*193/2], gpk [B][192]  the active normal equations in the solve kernel's skyline order (assembled by gather, no atomics)
+//   chol_plan           per distinct envelope: skyline row pointers and the Cholesky's trailing-update tiles per panel (int)
 //   Tvis [B][80*80], tvec [B][80]     Schur sums  sum_k gamma_k w_k w_k^T  and  sum_k gamma_k w_k gl_k
 //   per-window solver vectors (scale, D, scaled gradient, Gauss-Newton step) of length 192 + nlm
 #pragma once
@@ -74,6 +75,7 @@ struct WinMeta {        // read-only during a solve
     short tcol[NB];     // compact column of fixed block b, -1 if constant / absent / unreferenced
     short efirst[TFIX]; // envelope of the reduced system: first structurally non-zero column of compact row i (<= i)
     int esize;          // number of stored entries = sum_i (i - efirst[i] + 1)
+    int plan_off;       // the envelope's factorisation plan in chol_plan (kernels_solve.cuh; windows with one envelope share it)
     unsigned char flags[NB], mask[NB];
     double G[3], S_vis[4], w_plane[3], huber;
 };
@@ -125,6 +127,7 @@ struct BatchDev {       // passed by value to every kernel
     double *pair_out;               // [npitems_total][PAIR_OUT] tile (0,0), (0,1), (1,1) of G in mma.m8n8k4 accumulator order
     double *pair_red;               // [B][PAIR_RED] per frame: diagonal block (21) + gradient (6); per pair a < b: off-diagonal block (36)  (pair_reduce)
     const WinMeta *meta;
+    const int *chol_plan;           // factorisation plans of the batch's distinct envelopes (kernels_solve.cuh chol_plan_build), at WinMeta.plan_off
     WinWork *work;
     const PriorDev *prior;
     Opts opt;

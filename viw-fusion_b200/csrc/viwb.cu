@@ -19,6 +19,7 @@
 #include "kernels_fm.cuh"
 
 #include <algorithm>
+#include <map>
 #include <atomic>
 #include <chrono>
 #include <cstdio>
@@ -650,6 +651,25 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
             for (int f = 0; f < NFR; f++) if (lo.run_nt[f]) lo.run_slot[f] = (int)start[maxt - lo.run_nt[f]]++;
         }
     }
+    // factorisation plans (kernels_solve.cuh): one per distinct envelope, shared by the windows that have it -- the plan is a function of the
+    // envelope alone, so a window is factored the same way whatever else the batch holds
+    std::vector<std::vector<int>> plans;
+    size_t nplan = 0;
+    {
+        std::map<std::vector<short>, int> env_plan;
+        std::vector<int> env_of(B), env_win;
+        for (int w = 0; w < B; w++) {
+            const WinMeta &m = b->meta[w];
+            auto ins = env_plan.emplace(std::vector<short>(m.efirst, m.efirst + m.nf), (int)env_win.size());
+            if (ins.second) env_win.push_back(w);
+            env_of[w] = ins.first->second;
+        }
+        plans.resize(env_win.size());
+        parallel_for((int)env_win.size(), [&](int e) { const WinMeta &m = b->meta[env_win[e]]; chol_plan_build(m.efirst, m.nf, plans[e]); });
+        std::vector<int> off(plans.size());
+        for (size_t e = 0; e < plans.size(); e++) { off[e] = (int)nplan; nplan += plans[e].size(); }
+        for (int w = 0; w < B; w++) b->meta[w].plan_off = off[env_of[w]];
+    }
     // ---- phase 2: offsets
     size_t nlmb = 0, npit = 0, nxr = 0, nmpit = 0, nmxr = 0;      // nxr / nmxr: record regions in DOUBLES (solver / marginalisation share one buffer)
     size_t nobsi = 0;
@@ -669,7 +689,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
         b->algorithmic_bytes += window_algorithmic_bytes(p, opt->max_num_iterations);
     }
     for (int w = 0; w < B; w++) { WinMeta &m = b->meta[w]; m.mitem_off = (int)nit_m; nit_m += m.nmitems; m.mlist_off = (int)nlist; nlist += low[w].nlist_m; }
-    if (nxr > 0x7fffffff || nmxr > 0x7fffffff || nstate > 0x7fffffff || nvis * 12 > 0x7fffffffull * 4 || nlist > 0x7fffffff) { batch_free(ctx, b); return fail(ctx, VIWB_ERR_INVALID, "batch too large"); }
+    if (nxr > 0x7fffffff || nmxr > 0x7fffffff || nstate > 0x7fffffff || nvis * 12 > 0x7fffffffull * 4 || nlist > 0x7fffffff || nplan > 0x7fffffff) { batch_free(ctx, b); return fail(ctx, VIWB_ERR_INVALID, "batch too large"); }
     std::vector<PriorDev> priors(npri);
     for (int w = 0; w < B; w++) if (b->meta[w].prior_idx >= 0) {
         const viwb_prior &pr = *problems[w].prior; PriorDev &pd = priors[b->meta[w].prior_idx]; memset(&pd, 0, sizeof pd);
@@ -706,6 +726,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     IN(&bd.prior_J, h.prior_J, npJ); IN(&bd.prior_r, h.prior_r, npr); IN(&bd.prior_x0, h.prior_x0, npri * SFIX); IN(&bd.x_init, h.x_init, nstate); IN(&b->work_init_dev, h.work, B);
     IN(&bd.vis_pos, h.vis_pos, bd.n_fused_wide ? nvis : 0); IN(&bd.lmb_desc, h.lmb_desc, nlmb); IN(&bd.pitems, h.pitems, npit);
     IN(&bd.mvis_pos, h.mvis_pos, nmpit ? nvis : 0); IN(&bd.mpitems, h.mpitems, nmpit);
+    int *h_plan = nullptr; IN(&bd.chol_plan, h_plan, nplan);
     IN(&bd.run_desc, h.run_desc, nrun); IN(&bd.run_tile, h.run_tile, nrtile); IN(&bd.run_f, h.run_f, nrun ? nvis : 0); IN(&bd.run_lm, h.run_lm, nrun ? 2 * nlm : 0);
     const size_t nvec = (size_t)B * TFIX + nlm;
     const bool any_unfused = bd.n_unfused || bd.n_munfused;      // lin_vis' per-factor records and costs
@@ -741,6 +762,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     h.nitems_solve_total = (int)nit_s;
     if (npri) memcpy(h.prior, priors.data(), sizeof(PriorDev) * npri);
     h.lm_fptr[nlm] = (int)nvis;
+    for (const std::vector<int> &pl : plans) { memcpy(h_plan, pl.data(), sizeof(int) * pl.size()); h_plan += pl.size(); }
     // ---- phase 3 (parallel): fill
     std::vector<unsigned char> obs_viol(B, 0); h.obs_viol = obs_viol.data();
     parallel_for(B, [&](int w) { lower_fill(problems[w], states[w], w, b->meta[w], low[w], h, opt->initial_trust_region_radius); });
