@@ -55,8 +55,8 @@ static void emu_launch(F f, const BatchDev &bd, int gx, int gy, size_t smem_byte
 #endif
     for (int by = 0; by < gy; by++) for (int bx = 0; bx < gx; bx++) f(bd, bx, by, 0, 1, sm.data(), mode);
 }
-#define LAUNCH(name, bd, gx, gy, nt, smem_bytes, mode, stream) emu_launch(name##_block, bd, gx, gy, smem_bytes, mode)
 #define NT(n) 1
+enum { PRE_WPB = 1 };      // warps per block of the pre-integration kernels (kernels_preint.cuh): one per emulated block
 #else
 #include <cuda_runtime.h>
 typedef cudaStream_t stream_t;
@@ -124,10 +124,21 @@ DEF_KERNEL2(marg_tri, MARG_TRI_NT, 3)
 DEF_KERNEL(marg_ql, 32)
 DEF_KERNEL2(marg_apply, 128, 4)
 DEF_KERNEL(outlier, 128)
-#define LAUNCH(name, bd, gx, gy, nt, smem_bytes, mode, stream) \
-    do { if ((gx) > 0 && (gy) > 0) { g_prof.begin((mode) == 1 ? #name "_marg" : #name, stream); name##_kernel<<<dim3((gx), (gy)), (nt), (smem_bytes), (stream)>>>(bd, mode); g_prof.end(stream); } } while (0)
 #define NT(n) (n)
 #endif
+// Every kernel launch goes through KERNEL.  An empty grid launches nothing.  Otherwise the library issues kernel<<<(gx, gy), nt, smem>>>args on the
+// context's stream inside the profiler's bracket, and the emulation build runs the statements of the variadic tail instead (block functions called
+// block by block, one host thread per block: the grids of the emulation are sized with NT(n) = 1).  Either way ctx->launches counts exactly the
+// launches issued, so viwb_launch_count equals the sum of the profile's launches.
+#ifdef VIWB_HOST_EMU
+#define KERNEL(ctx, pname, gx, gy, nt, smem, kernel, args, ...) do { if ((gx) > 0 && (gy) > 0) { __VA_ARGS__; (ctx)->launches++; } } while (0)
+#else
+#define KERNEL(ctx, pname, gx, gy, nt, smem, kernel, args, ...) \
+    do { if ((gx) > 0 && (gy) > 0) { g_prof.begin(pname, (ctx)->stream); kernel<<<dim3((gx), (gy)), (nt), (smem), (ctx)->stream>>> args; g_prof.end((ctx)->stream); (ctx)->launches++; } } while (0)
+#endif
+// the BatchDev kernels (DEF_KERNEL): name##_kernel in the library, name##_block in the emulation; profiled as name, or name_marg in mode 1
+#define LAUNCH(ctx, name, bd, gx, gy, nt, smem_bytes, mode) \
+    KERNEL(ctx, (mode) == 1 ? #name "_marg" : #name, gx, gy, nt, smem_bytes, name##_kernel, (bd, mode), emu_launch(name##_block, bd, gx, gy, smem_bytes, mode))
 
 // one device slab + one pinned host staging slab; cached in the context so that the host-buffer entry points do not
 // pay cudaMalloc / cudaHostAlloc on every call
@@ -160,6 +171,69 @@ static inline void bind_device(const viwb_context *ctx) {
 #endif
 }
 #define CK(call) do { int e_ = (call); if (e_) return fail(ctx, VIWB_ERR_CUDA, std::string(#call) + ": " + dev_errstr(e_)); } while (0)
+// the error of a launch that failed at issue time (a bad configuration, no kernel image for the device); every entry point that launches asks once
+static int launch_status(viwb_context *ctx) {
+#ifndef VIWB_HOST_EMU
+    const int e = (int)cudaGetLastError();
+    if (e) return fail(ctx, VIWB_ERR_CUDA, std::string("kernel launch: ") + dev_errstr(e));
+#endif
+    (void)ctx;
+    return VIWB_OK;
+}
+// the kernels' dynamic shared memory above the default limit; cudaFuncSetAttribute applies to the current device, so once per context
+static int ensure_attrs(viwb_context *ctx) {
+#ifndef VIWB_HOST_EMU
+    if (!ctx->attrs_set) {
+        CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_NT, TFIX * (TFIX + 1) / 2) * 8)));
+        CK(cudaFuncSetAttribute(lin_vis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_smem_doubles(128) * 8)));
+        CK(cudaFuncSetAttribute(lin_vis_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_run_smem_doubles() * 8)));
+        CK(cudaFuncSetAttribute(lin_vis_lm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_lm_smem_doubles(true) * 8)));
+        CK(cudaFuncSetAttribute(syrk_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(syrk_mma_smem_doubles() * 8)));
+        CK(cudaFuncSetAttribute(marg_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_prep_smem_doubles(256, 100) * 8)));
+        CK(cudaFuncSetAttribute(marg_tri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_eig_smem_doubles(256, 100) * 8)));
+        CK(cudaFuncSetAttribute(marg_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_apply_smem_doubles(128, 100) * 8)));
+        CK(cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_eig_smem_doubles(256, 100) * 8)));
+        CK(cudaFuncSetAttribute(det_corners_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)det_tile_smem_bytes()));
+        CK(cudaFuncSetAttribute(det_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)det_select_smem_bytes()));
+        ctx->attrs_set = true;
+    }
+#endif
+    (void)ctx;
+    return 0;
+}
+
+static size_t align_up(size_t v) { return (v + 255) & ~(size_t)255; }
+
+// One buffer of a one-shot entry point (staged): an input uploaded before the launch, an output downloaded after it, or device scratch.  `dev`
+// is the kernel argument that receives the device address; an input or output without a host pointer is neither allocated nor copied (NULL).
+struct Stage { void **dev; const void *in; void *out; size_t bytes; bool scratch; };
+template <typename T> static Stage stage_in(T *&dev, const void *host, size_t bytes) { return {(void **)&dev, host, nullptr, bytes, false}; }
+template <typename T> static Stage stage_out(T *&dev, void *host, size_t bytes) { return {(void **)&dev, nullptr, host, bytes, false}; }
+template <typename T> static Stage stage_tmp(T *&dev, size_t bytes) { return {(void **)&dev, nullptr, nullptr, bytes, true}; }
+// A one-shot entry point: one device block laid out align_up-aligned, the inputs up, launch() (KERNEL calls), the outputs down, then synchronise
+// before the block is freed.  Copies run in the order of `bufs`.
+template <typename Launch> static int staged(viwb_context *ctx, const char *what, std::initializer_list<Stage> bufs, Launch launch) {
+    bind_device(ctx);
+    size_t tot = 0;
+    for (const Stage &b : bufs) if (b.scratch || b.in || b.out) tot += align_up(b.bytes);
+    char *d = nullptr;
+    int e = dev_malloc((void **)&d, tot), rc = VIWB_OK;
+    if (e) return fail(ctx, VIWB_ERR_CUDA, std::string(what) + ": " + dev_errstr(e));
+    size_t o = 0;
+    for (const Stage &b : bufs) {
+        const bool used = b.scratch || b.in || b.out;
+        *b.dev = used ? d + o : nullptr;
+        if (used) o += align_up(b.bytes);
+        if (b.in && !e) e = dev_h2d(*b.dev, b.in, b.bytes, ctx->stream);
+    }
+    if (!e) { launch(); rc = launch_status(ctx); }
+    for (const Stage &b : bufs) if (b.out && !e && !rc) e = dev_d2h(b.out, *b.dev, b.bytes, ctx->stream);
+    const int es = dev_sync(ctx->stream);
+    if (!e) e = es;
+    dev_free(d);
+    if (rc) return rc;
+    return e ? fail(ctx, VIWB_ERR_CUDA, std::string(what) + ": " + dev_errstr(e)) : VIWB_OK;
+}
 
 #include "lk_host.inl"
 #include "detect_host.inl"
@@ -186,8 +260,6 @@ struct viwb_batch {
     int max_iter;
     double max_time;       // max_solver_time_in_seconds (0 = off): checked on the host between rounds, like Ceres' wall-clock test
 };
-
-static size_t align_up(size_t v) { return (v + 255) & ~(size_t)255; }
 
 static void opts_from(const viwb_options *o, Opts &d) {
     d.max_num_iterations = o->max_num_iterations; d.max_invalid = o->max_num_consecutive_invalid_steps; d.jacobi_scaling = o->jacobi_scaling;
@@ -773,29 +845,12 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     const double t_filled = now_ms();
     { int e = dev_h2d(ar->dev, ar->host, in_bytes, ctx->stream); if (e) { batch_free(ctx, b); return fail(ctx, VIWB_ERR_CUDA, std::string("H2D: ") + dev_errstr(e)); } }
     ctx->h2d_bytes += (long long)in_bytes;
-    if (nvis) { LAUNCH(vis_expand, bd, B, 1, NT(128), 0, 0, ctx->stream); ctx->launches++; }      // code words + split observations -> the tables the kernels read
+    if (nvis) LAUNCH(ctx, vis_expand, bd, B, 1, NT(128), 0, 0);      // code words + split observations -> the tables the kernels read
+    { const int rc = launch_status(ctx); if (rc) { batch_free(ctx, b); return rc; } }
     // (no wait here: the kernels of the run are queued behind the upload on the same stream, the results are staged in their own region of the slab, and the
     //  slab is next written by the host only after a fetch has synchronised)
     if (g_timing) fprintf(stderr, "[viwb] build B=%d: plan+slabs %.2f ms (count %.2f), fill %.2f ms (%.1f MB), h2d %.2f ms\n", B, t_alloc - t_start, t_counted - t_start, t_filled - t_alloc, in_bytes / 1e6, now_ms() - t_filled);
     *out = b;
-    return 0;
-}
-
-static int ensure_attrs(viwb_context *ctx) {
-#ifndef VIWB_HOST_EMU
-    if (!ctx->attrs_set) {
-        CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_NT, TFIX * (TFIX + 1) / 2) * 8)));
-        CK(cudaFuncSetAttribute(lin_vis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_smem_doubles(128) * 8)));
-        CK(cudaFuncSetAttribute(lin_vis_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_run_smem_doubles() * 8)));
-        CK(cudaFuncSetAttribute(lin_vis_lm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_lm_smem_doubles(true) * 8)));
-        CK(cudaFuncSetAttribute(syrk_mma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(syrk_mma_smem_doubles() * 8)));
-        CK(cudaFuncSetAttribute(marg_prep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_prep_smem_doubles(256, 100) * 8)));
-        CK(cudaFuncSetAttribute(marg_tri_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_eig_smem_doubles(256, 100) * 8)));
-        CK(cudaFuncSetAttribute(marg_apply_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_apply_smem_doubles(128, 100) * 8)));
-        CK(cudaFuncSetAttribute(marg_eig_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(marg_eig_smem_doubles(256, 100) * 8)));
-        ctx->attrs_set = true;
-    }
-#endif
     return 0;
 }
 
@@ -823,35 +878,28 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
         const bool solve = mode == MODE_SOLVE;
         const bool unfused = solve ? bd.n_unfused > 0 : bd.n_munfused > 0;      // windows outside the fused path (irregular factor tables)
         const int vmode = cost_only ? (int)MODE_COST : mode;
-        if (solve && bd.n_fused_compact > 0) { LAUNCH(lin_vis_lm, bd, bd.nrun_total, 1, NT(LMB_FACTORS), lin_vis_run_smem_doubles() * 8, vmode, st); ctx->launches++; }      // + the compact windows' pair chunks
-        if (solve ? bd.n_fused_wide > 0 : bd.n_mfused > 0) { LAUNCH(lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, vmode, st); ctx->launches++; }
+        if (solve && bd.n_fused_compact > 0) LAUNCH(ctx, lin_vis_lm, bd, bd.nrun_total, 1, NT(LMB_FACTORS), lin_vis_run_smem_doubles() * 8, vmode);      // + the compact windows' pair chunks
+        if (solve ? bd.n_fused_wide > 0 : bd.n_mfused > 0) LAUNCH(ctx, lin_vis_lm_wide, bd, bd.nlmb_total, 1, NT(LMB_FACTORS), lin_vis_lm_smem_doubles(true) * 8, vmode);
         if (unfused) {
-            LAUNCH(lin_vis, bd, g_vis, 1, nt_vis, lin_vis_smem_doubles(nt_vis) * 8, mode, st);
-            LAUNCH(lm_reduce, bd, g_lm, 1, nt_lm, 0, mode, st);
-            ctx->launches += (g_vis > 0) + (g_lm > 0);
+            LAUNCH(ctx, lin_vis, bd, g_vis, 1, nt_vis, lin_vis_smem_doubles(nt_vis) * 8, mode);
+            LAUNCH(ctx, lm_reduce, bd, g_lm, 1, nt_lm, 0, mode);
         }
-        LAUNCH(lin_small, bd, B, 1, nt_small, sm_small, mode, st); ctx->launches++;
+        LAUNCH(ctx, lin_small, bd, B, 1, nt_small, sm_small, mode);
         if (cost_only) return;
         const int nfi = solve ? bd.npitems_total : bd.nmpitems_total, wpb = nt_asm / (nt_asm < 32 ? nt_asm : 32);
         if (nfi > 0) {
-            if (!solve || bd.n_fused_wide > 0) { LAUNCH(asm_pairs_wide, bd, (nfi + wpb - 1) / wpb, 1, NT(128), 0, mode, st); ctx->launches++; }
-            LAUNCH(pair_reduce, bd, B, 1, NT(PAIR_RED_NT), (size_t)bd.pitems_max * sizeof(int), mode, st); ctx->launches++;
+            if (!solve || bd.n_fused_wide > 0) LAUNCH(ctx, asm_pairs_wide, bd, (nfi + wpb - 1) / wpb, 1, NT(128), 0, mode);
+            LAUNCH(ctx, pair_reduce, bd, B, 1, NT(PAIR_RED_NT), (size_t)bd.pitems_max * sizeof(int), mode);
         }
-        if (unfused) {
-            const int ni = solve ? bd.nitems_solve : bd.nitems_marg;
-            LAUNCH(asm_items, bd, (ni * ASM_SPLIT + wpb - 1) / wpb, 1, nt_asm, 0, mode, st);
-            ctx->launches += ni > 0;
-        }
-        LAUNCH(syrk_mma, bd, B, 1, NT(SYRK_NT), syrk_mma_smem_doubles() * 8, mode, st);
-        ctx->launches++;
+        if (unfused) LAUNCH(ctx, asm_items, bd, ((solve ? bd.nitems_solve : bd.nitems_marg) * ASM_SPLIT + wpb - 1) / wpb, 1, nt_asm, 0, mode);
+        LAUNCH(ctx, syrk_mma, bd, B, 1, NT(SYRK_NT), syrk_mma_smem_doubles() * 8, mode);
     };
     if (what & (RUN_SOLVE | RUN_MARG | RUN_LIN_ONLY)) {
         const int ns = bd.nimu_total + bd.nwheel_total, nt_s = NT(128);
-        LAUNCH(setup, bd, (ns + nt_s - 1) / nt_s, 1, nt_s, 0, 0, st);
-        LAUNCH(prior_setup, bd, bd.nprior, 1, NT(256), 0, 0, st);
-        ctx->launches += (ns > 0) + (bd.nprior > 0);
+        LAUNCH(ctx, setup, bd, (ns + nt_s - 1) / nt_s, 1, nt_s, 0, 0);
+        LAUNCH(ctx, prior_setup, bd, bd.nprior, 1, NT(256), 0, 0);
     }
-    if (what & RUN_LIN_ONLY) { lin(MODE_SOLVE, false); LAUNCH(solve, bd, B, 1, nt_solve, sm_solve, 2, st); ctx->launches++; }
+    if (what & RUN_LIN_ONLY) { lin(MODE_SOLVE, false); LAUNCH(ctx, solve, bd, B, 1, nt_solve, sm_solve, 2); }
     if (what & RUN_SOLVE) {
         // SOLVER_TIME (estimator.cpp:1650-1653): Ceres tests the wall clock after every iteration; here the host
         // waits for each round only when a limit is set, and the round after the limit just decides the pending
@@ -864,26 +912,21 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
                 last = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count() >= b->max_time;
             }
             lin(MODE_SOLVE, last || (round == b->max_iter && round > 0));
-            LAUNCH(solve, bd, B, 1, nt_solve, sm_solve, last ? 3 : 0, st);
-            ctx->launches++;
+            LAUNCH(ctx, solve, bd, B, 1, nt_solve, sm_solve, last ? 3 : 0);
         }
     }
-    if (what & RUN_REANCHOR) { LAUNCH(reanchor, bd, B, 1, NT(32), 0, 0, st); ctx->launches++; }
+    if (what & RUN_REANCHOR) LAUNCH(ctx, reanchor, bd, B, 1, NT(32), 0, 0);
     if ((what & RUN_MARG) && b->any_marg) {
         lin(MODE_MARG, false);
-        LAUNCH(marg_prep, bd, B, 1, nt_marg, sm_marg, 0, st);
-        if (g_marg_one_kernel) { LAUNCH(marg_eig, bd, B, 1, nt_marg, sm_eig, 0, st); ctx->launches += 2; }
+        LAUNCH(ctx, marg_prep, bd, B, 1, nt_marg, sm_marg, 0);
+        if (g_marg_one_kernel) LAUNCH(ctx, marg_eig, bd, B, 1, nt_marg, sm_eig, 0);
         else {
-            LAUNCH(marg_tri, bd, B, 1, NT(MARG_TRI_NT), sm_eig, 0, st);
-            LAUNCH(marg_ql, bd, B, 1, NT(32), 2 * MAXPRI * 8, 0, st);
-            LAUNCH(marg_apply, bd, B, 1, NT(128), marg_apply_smem_doubles(128, bd.marg_nmax) * 8, 0, st);
-            ctx->launches += 4;
+            LAUNCH(ctx, marg_tri, bd, B, 1, NT(MARG_TRI_NT), sm_eig, 0);
+            LAUNCH(ctx, marg_ql, bd, B, 1, NT(32), 2 * MAXPRI * 8, 0);
+            LAUNCH(ctx, marg_apply, bd, B, 1, NT(128), marg_apply_smem_doubles(128, bd.marg_nmax) * 8, 0);
         }
     }
-#ifndef VIWB_HOST_EMU
-    CK((int)cudaGetLastError());
-#endif
-    return 0;
+    return launch_status(ctx);
 }
 
 static int batch_fetch(viwb_context *ctx, viwb_batch *b, double *const *states, viwb_summary *summaries, viwb_prior *priors_out) {
@@ -1075,8 +1118,8 @@ extern "C" int viwb_batch_outliers(viwb_context *ctx, viwb_batch *b, double foca
     bind_device(ctx);
     BatchDev bd = b->bd; bd.out_focal = focal_length; bd.out_thresh = threshold_px;
     const int nt = NT(128);
-    LAUNCH(outlier, bd, (bd.nlm_total + nt - 1) / nt, 1, nt, 0, 0, ctx->stream);
-    ctx->launches += bd.nlm_total > 0;
+    LAUNCH(ctx, outlier, bd, (bd.nlm_total + nt - 1) / nt, 1, nt, 0, 0);
+    const int rc = launch_status(ctx); if (rc) return rc;
     std::vector<int> h(bd.nlm_total > 0 ? bd.nlm_total : 1);
     CK(dev_d2h(h.data(), bd.lm_outlier, (size_t)bd.nlm_total * sizeof(int), ctx->stream));
     CK(dev_sync(ctx->stream));
@@ -1225,7 +1268,6 @@ __global__ void eval_factor_kernel(EvalArgs a) { if (threadIdx.x == 0 && blockId
 
 extern "C" int viwb_factor_evaluate(viwb_context *ctx, int type, const viwb_globals *gl, const double *consts, const double *const *params,
                                     double *residuals, double **jacobians) {
-    bind_device(ctx);
     if (!ctx || !gl || !params || !residuals || type < 0 || type > 5) return VIWB_ERR_INVALID;
     static const int nblk[6] = {5, 6, 4, 4, 7, 4};
     static const int sizes[6][7] = {{7, 7, 7, 1, 1, 0, 0}, {7, 7, 7, 7, 1, 1, 0}, {7, 7, 1, 1, 0, 0, 0}, {7, 9, 7, 9, 0, 0, 0}, {7, 7, 7, 1, 1, 1, 1}, {7, 7, 4, 1, 0, 0, 0}};
@@ -1238,18 +1280,11 @@ extern "C" int viwb_factor_evaluate(viwb_context *ctx, int type, const viwb_glob
     in[10] = gl->huber_delta;
     if (ncons[type]) { if (!consts) return VIWB_ERR_INVALID; memcpy(in.data() + 11, consts, sizeof(double) * ncons[type]); }
     for (int i = 0; i < nblk[type]; i++) memcpy(in.data() + 11 + 287 + 9 * i, params[i], sizeof(double) * sizes[type][i]);
-    double *din = nullptr, *dout = nullptr;
-    CK(dev_malloc((void **)&din, in.size() * 8)); CK(dev_malloc((void **)&dout, out.size() * 8));
-    CK(dev_h2d(din, in.data(), in.size() * 8, ctx->stream));
-    EvalArgs a; a.type = type; a.want_j = jacobians ? 1 : 0; a.in = din; a.out = dout;
-#ifdef VIWB_HOST_EMU
-    eval_factor_device(a);
-#else
-    eval_factor_kernel<<<1, 32, 0, ctx->stream>>>(a);
-#endif
-    ctx->launches++;
-    CK(dev_d2h(out.data(), dout, out.size() * 8, ctx->stream)); CK(dev_sync(ctx->stream));
-    dev_free(din); dev_free(dout);
+    EvalArgs a; a.type = type; a.want_j = jacobians ? 1 : 0;
+    const int rc = staged(ctx, "factor_evaluate", {stage_in(a.in, in.data(), in.size() * 8), stage_out(a.out, out.data(), out.size() * 8)}, [&] {
+        KERNEL(ctx, "eval_factor", 1, 1, 32, 0, eval_factor_kernel, (a), eval_factor_device(a));
+    });
+    if (rc) return rc;
     for (int i = 0; i < nres[type]; i++) residuals[i] = out[i];
     if (jacobians) {   // formatting only: tangent columns -> the reference's row-major (rows x global size) blocks, last pose column zero
         const double *J = out.data() + 15;
@@ -1286,31 +1321,16 @@ VIWB_D void prior_eval_device(const PriorEvalArgs &a, int tid, int nt, double *d
 __global__ void prior_eval_kernel(PriorEvalArgs a) { __shared__ double dx[MAXPRI]; prior_eval_device(a, threadIdx.x, blockDim.x, dx); }
 #endif
 extern "C" int viwb_prior_evaluate(viwb_context *ctx, const viwb_prior *prior, const double *state, double *residuals, double *jacobian) {
-    bind_device(ctx);
     if (!ctx || !prior || !state || !residuals || prior->n <= 0 || prior->n > MAXPRI) return VIWB_ERR_INVALID;
     const int n = prior->n;
-    double *d = nullptr;
-    const size_t tot = (size_t)n * n + n + SFIX + SFIX + n;
-    CK(dev_malloc((void **)&d, tot * 8));
-    {   int e = dev_h2d(d, prior->J, (size_t)n * n * 8, ctx->stream);
-        if (!e) e = dev_h2d(d + (size_t)n * n, prior->r, n * 8, ctx->stream);
-        if (!e) e = dev_h2d(d + (size_t)n * n + n, prior->x0, SFIX * 8, ctx->stream);
-        if (!e) e = dev_h2d(d + (size_t)n * n + n + SFIX, state, SFIX * 8, ctx->stream);
-        if (e) { dev_free(d); return fail(ctx, VIWB_ERR_CUDA, std::string("prior upload: ") + dev_errstr(e)); } }
     PriorEvalArgs a; memset(&a, 0, sizeof a);
     a.p.n = n; a.p.nb = prior->num_blocks;
     for (int i = 0; i < prior->num_blocks; i++) { a.p.block_id[i] = prior->block_id[i]; a.p.block_idx[i] = prior->block_idx[i]; }
-    a.J = d; a.r = d + (size_t)n * n; a.x0 = a.r + n; a.x = a.x0 + SFIX; a.res = d + (size_t)n * n + n + 2 * SFIX;
-#ifdef VIWB_HOST_EMU
-    { double dx[MAXPRI]; prior_eval_device(a, 0, 1, dx); }
-#else
-    prior_eval_kernel<<<1, 128, 0, ctx->stream>>>(a);
-#endif
-    ctx->launches++;
-    {   int e = dev_d2h(residuals, a.res, n * 8, ctx->stream);
-        if (!e) e = dev_sync(ctx->stream);
-        dev_free(d);
-        if (e) return fail(ctx, VIWB_ERR_CUDA, std::string("prior download: ") + dev_errstr(e)); }
+    const int rc = staged(ctx, "prior_evaluate", {stage_in(a.J, prior->J, (size_t)n * n * 8), stage_in(a.r, prior->r, (size_t)n * 8), stage_in(a.x0, prior->x0, SFIX * 8),
+                                                  stage_in(a.x, state, SFIX * 8), stage_out(a.res, residuals, (size_t)n * 8)}, [&] {
+        KERNEL(ctx, "prior_eval", 1, 1, 128, 0, prior_eval_kernel, (a), double dx[MAXPRI]; prior_eval_device(a, 0, 1, dx));
+    });
+    if (rc) return rc;
     if (jacobian) {   // formatting only (marginalization_factor.cpp:381-394): J_lin columns at the block's state offset
         memset(jacobian, 0, sizeof(double) * n * SFIX);
         for (int i = 0; i < prior->num_blocks; i++) {
@@ -1322,37 +1342,10 @@ extern "C" int viwb_prior_evaluate(viwb_context *ctx, const viwb_prior *prior, c
 }
 
 // -------------------------------------------------------------------------------------- pre-integration (SURVEY 8 f-2)
-template <typename Args, typename EmuFn>
-static int preint_run(viwb_context *ctx, Args &a, int n, const int32_t *counts, const double *dt, const double *s0, const double *s1, int rec_doubles, double *records,
-                      const double *const *extra, const int *extra_doubles, int nextra, const double **dev_extra, EmuFn emu, int smem_doubles, bool imu) {
-    bind_device(ctx);
-    std::vector<int> off(n + 1, 0);
+// interval i owns counts[i] steps of dt and counts[i] + 1 rows of samples; off: the first step of every interval
+static int preint_offsets(viwb_context *ctx, int n, const int32_t *counts, std::vector<int> &off) {
+    off.assign(n + 1, 0);
     for (int i = 0; i < n; i++) { if (counts[i] < 0) return fail(ctx, VIWB_ERR_INVALID, "negative sample count"); off[i + 1] = off[i] + counts[i]; }
-    const size_t steps = off[n], rows = steps + n;
-    size_t bytes = align_up((n + 1) * sizeof(int)) + align_up(steps * 8) + 2 * align_up(rows * 24) + align_up((size_t)n * rec_doubles * 8);
-    for (int k = 0; k < nextra; k++) bytes += align_up((size_t)n * extra_doubles[k] * 8);
-    char *d = nullptr;
-    CK(dev_malloc((void **)&d, bytes));
-    size_t o = 0;
-    int *d_off = (int *)(d + o); o += align_up((n + 1) * sizeof(int));
-    double *d_dt = (double *)(d + o); o += align_up(steps * 8);
-    double *d_s0 = (double *)(d + o); o += align_up(rows * 24);
-    double *d_s1 = (double *)(d + o); o += align_up(rows * 24);
-    double *d_rec = (double *)(d + o); o += align_up((size_t)n * rec_doubles * 8);
-    int e = dev_h2d(d_off, off.data(), (n + 1) * sizeof(int), ctx->stream);
-    if (!e) e = dev_h2d(d_dt, dt, steps * 8, ctx->stream);
-    if (!e) e = dev_h2d(d_s0, s0, rows * 24, ctx->stream);
-    if (!e) e = dev_h2d(d_s1, s1, rows * 24, ctx->stream);
-    for (int k = 0; k < nextra && !e; k++) { double *p = (double *)(d + o); o += align_up((size_t)n * extra_doubles[k] * 8); e = dev_h2d(p, extra[k], (size_t)n * extra_doubles[k] * 8, ctx->stream); dev_extra[k] = p; }
-    if (e) { dev_free(d); return fail(ctx, VIWB_ERR_CUDA, "pre-integration upload failed"); }
-    a.n = n; a.off = d_off; a.dt = d_dt; a.rec = d_rec;
-    emu(a, d_s0, d_s1);
-    (void)smem_doubles; (void)imu;
-    ctx->launches++;
-    e = dev_d2h(records, d_rec, (size_t)n * rec_doubles * 8, ctx->stream);
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(d);
-    if (e) return fail(ctx, VIWB_ERR_CUDA, "pre-integration download failed");
     return VIWB_OK;
 }
 
@@ -1360,98 +1353,58 @@ extern "C" int viwb_imu_preintegrate(viwb_context *ctx, int n, const int32_t *co
                                      const double *ba, const double *bg, const double *noise, double *records) {
     if (!ctx || n < 0 || !counts || !dt || !acc || !gyr || !ba || !bg || !noise || !records) return VIWB_ERR_INVALID;
     if (n == 0) return VIWB_OK;
-    ImuPreArgs a; for (int k = 0; k < 4; k++) a.noise[k] = noise[k];
-    const double *extra[2] = {ba, bg}; const int ed[2] = {3, 3}; const double *dv[2] = {nullptr, nullptr};
-    stream_t st = ctx->stream;
-    return preint_run(ctx, a, n, counts, dt, acc, gyr, 287, records, extra, ed, 2, dv, [&](ImuPreArgs &q, const double *d0, const double *d1) {
-        q.acc = d0; q.gyr = d1; q.ba = dv[0]; q.bg = dv[1];
-#ifdef VIWB_HOST_EMU
-        std::vector<double> sm(PRE_IMU_SMEM); for (int i = 0; i < q.n; i++) imu_preint_warp(q, i, 0, 1, sm.data());
-#else
-        g_prof.begin("imu_preint", st); imu_preint_kernel<<<(q.n + PRE_WPB - 1) / PRE_WPB, 32 * PRE_WPB, PRE_WPB * PRE_IMU_SMEM * 8, st>>>(q); g_prof.end(st);
-#endif
-    }, PRE_IMU_SMEM, true);
+    std::vector<int> off; const int rc = preint_offsets(ctx, n, counts, off); if (rc) return rc;
+    const size_t steps = off[n], rows = steps + n;
+    ImuPreArgs a; a.n = n; for (int k = 0; k < 4; k++) a.noise[k] = noise[k];
+    return staged(ctx, "imu_preintegrate", {stage_in(a.off, off.data(), off.size() * 4), stage_in(a.dt, dt, steps * 8), stage_in(a.acc, acc, rows * 24), stage_in(a.gyr, gyr, rows * 24),
+                                            stage_in(a.ba, ba, (size_t)n * 24), stage_in(a.bg, bg, (size_t)n * 24), stage_out(a.rec, records, (size_t)n * 287 * 8)}, [&] {
+        KERNEL(ctx, "imu_preint", (n + PRE_WPB - 1) / PRE_WPB, 1, 32 * PRE_WPB, PRE_WPB * PRE_IMU_SMEM * 8, imu_preint_kernel, (a),
+               std::vector<double> sm(PRE_IMU_SMEM); for (int i = 0; i < n; i++) imu_preint_warp(a, i, 0, 1, sm.data()));
+    });
 }
 extern "C" int viwb_wheel_preintegrate(viwb_context *ctx, int n, const int32_t *counts, const double *dt, const double *vel, const double *gyr,
                                        const double *s, const double *td, const double *noise, double *records) {
     if (!ctx || n < 0 || !counts || !dt || !vel || !gyr || !s || !td || !noise || !records) return VIWB_ERR_INVALID;
     if (n == 0) return VIWB_OK;
-    WheelPreArgs a; a.noise[0] = noise[0]; a.noise[1] = noise[1];
-    const double *extra[2] = {s, td}; const int ed[2] = {3, 1}; const double *dv[2] = {nullptr, nullptr};
-    stream_t st = ctx->stream;
-    return preint_run(ctx, a, n, counts, dt, vel, gyr, 78, records, extra, ed, 2, dv, [&](WheelPreArgs &q, const double *d0, const double *d1) {
-        q.vel = d0; q.gyr = d1; q.s = dv[0]; q.td = dv[1];
-#ifdef VIWB_HOST_EMU
-        std::vector<double> sm(PRE_WHEEL_SMEM); for (int i = 0; i < q.n; i++) wheel_preint_warp(q, i, 0, 1, sm.data());
-#else
-        g_prof.begin("wheel_preint", st); wheel_preint_kernel<<<(q.n + PRE_WPB - 1) / PRE_WPB, 32 * PRE_WPB, PRE_WPB * PRE_WHEEL_SMEM * 8, st>>>(q); g_prof.end(st);
-#endif
-    }, PRE_WHEEL_SMEM, false);
+    std::vector<int> off; const int rc = preint_offsets(ctx, n, counts, off); if (rc) return rc;
+    const size_t steps = off[n], rows = steps + n;
+    WheelPreArgs a; a.n = n; a.noise[0] = noise[0]; a.noise[1] = noise[1];
+    return staged(ctx, "wheel_preintegrate", {stage_in(a.off, off.data(), off.size() * 4), stage_in(a.dt, dt, steps * 8), stage_in(a.vel, vel, rows * 24), stage_in(a.gyr, gyr, rows * 24),
+                                              stage_in(a.s, s, (size_t)n * 24), stage_in(a.td, td, (size_t)n * 8), stage_out(a.rec, records, (size_t)n * 78 * 8)}, [&] {
+        KERNEL(ctx, "wheel_preint", (n + PRE_WPB - 1) / PRE_WPB, 1, 32 * PRE_WPB, PRE_WPB * PRE_WHEEL_SMEM * 8, wheel_preint_kernel, (a),
+               std::vector<double> sm(PRE_WHEEL_SMEM); for (int i = 0; i < n; i++) wheel_preint_warp(a, i, 0, 1, sm.data()));
+    });
 }
 
 // -------------------------------------------------------------------------------------- initialisation alignment (SURVEY 8 f-4 ii)
-struct InitWork { char *d = nullptr; double *R, *T, *imu, *wheel, *A, *b, *x, *out; int *perm; };
-static int init_work(viwb_context *ctx, InitWork &w, int F, const double *R, const double *T, const double *imu, const double *wheel) {
-    const int n = 3 * F + 4;
-    const size_t sR = align_up((size_t)F * 72), sT = align_up((size_t)F * 24), sI = align_up((size_t)(F - 1) * VIWB_IMU_DOUBLES * 8), sW = align_up((size_t)(F - 1) * VIWB_WHEEL_DOUBLES * 8);
-    const size_t sA = align_up((size_t)2 * n * n * 8), sv = align_up((size_t)(n + 8) * 8);
-    if (dev_malloc((void **)&w.d, sR + sT + sI + sW + sA + 3 * sv + align_up((size_t)n * 4))) return 1;
-    size_t o = 0;
-    w.R = (double *)(w.d + o); o += sR; w.T = (double *)(w.d + o); o += sT; w.imu = (double *)(w.d + o); o += sI; w.wheel = (double *)(w.d + o); o += sW;
-    w.A = (double *)(w.d + o); o += sA; w.b = (double *)(w.d + o); o += sv; w.x = (double *)(w.d + o); o += sv; w.out = (double *)(w.d + o); o += sv;
-    w.perm = (int *)(w.d + o);
-    int e = dev_h2d(w.R, R, (size_t)F * 72, ctx->stream);
-    if (!e && T) e = dev_h2d(w.T, T, (size_t)F * 24, ctx->stream);
-    if (!e) e = dev_h2d(w.imu, imu, (size_t)(F - 1) * VIWB_IMU_DOUBLES * 8, ctx->stream);
-    if (!e && wheel) e = dev_h2d(w.wheel, wheel, (size_t)(F - 1) * VIWB_WHEEL_DOUBLES * 8, ctx->stream);
-    return e;
-}
-
+// the normal equations of both solves: A (two n x n matrices: linear alignment factors a copy), b, x, the pivots; n = 3 F + 4
 extern "C" int viwb_solve_gyroscope_bias(viwb_context *ctx, int num_frames, const double *R, const double *imu_data, double *delta_bg) {
     if (!ctx || !R || !imu_data || !delta_bg) return VIWB_ERR_INVALID;
     if (num_frames < 2 || num_frames > VIWB_MAX_INIT_FRAMES) return fail(ctx, VIWB_ERR_INVALID, "solve_gyroscope_bias: 2..VIWB_MAX_INIT_FRAMES frames");
-    bind_device(ctx);
-    InitWork w; int e = init_work(ctx, w, num_frames, R, nullptr, imu_data, nullptr);
-    if (!e) {
-        GyroBiasArgs a; a.F = num_frames; a.R = w.R; a.imu = w.imu; a.A = w.A; a.b = w.b; a.x = w.x; a.perm = w.perm; a.out = w.out;
-#ifdef VIWB_HOST_EMU
-        gyro_bias_block(a, 0, 1);
-#else
-        g_prof.begin("gyro_bias", ctx->stream); gyro_bias_kernel<<<1, 32, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
-#endif
-        ctx->launches++;
-        e = dev_d2h(delta_bg, w.out, 24, ctx->stream);
-    }
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(w.d);
-    return e ? fail(ctx, VIWB_ERR_CUDA, "solve_gyroscope_bias failed") : VIWB_OK;
+    const int F = num_frames, n = 3 * F + 4;
+    GyroBiasArgs a; a.F = F;
+    return staged(ctx, "solve_gyroscope_bias", {stage_in(a.R, R, (size_t)F * 72), stage_in(a.imu, imu_data, (size_t)(F - 1) * VIWB_IMU_DOUBLES * 8), stage_tmp(a.A, (size_t)2 * n * n * 8),
+                                                stage_tmp(a.b, (size_t)(n + 8) * 8), stage_tmp(a.x, (size_t)(n + 8) * 8), stage_tmp(a.perm, (size_t)n * 4), stage_out(a.out, delta_bg, 24)}, [&] {
+        KERNEL(ctx, "gyro_bias", 1, 1, 32, 0, gyro_bias_kernel, (a), gyro_bias_block(a, 0, 1));
+    });
 }
 
 extern "C" int viwb_linear_alignment(viwb_context *ctx, int num_frames, const double *R, const double *T, const double *imu_data, const double *wheel_data,
                                      const double *tic, const double *rio, const double *tio, double g_norm, double *g, double *x, int32_t *x_size, int32_t *aligned) {
     if (!ctx || !R || !T || !imu_data || !tic || !g || !x || !x_size || !aligned || (wheel_data && (!rio || !tio))) return VIWB_ERR_INVALID;
     if (num_frames < 2 || num_frames > VIWB_MAX_INIT_FRAMES) return fail(ctx, VIWB_ERR_INVALID, "linear_alignment: 2..VIWB_MAX_INIT_FRAMES frames");
-    bind_device(ctx);
-    const int n = 3 * num_frames + 4;
-    InitWork w; int e = init_work(ctx, w, num_frames, R, T, imu_data, wheel_data);
-    std::vector<double> out((size_t)n + 8);
-    if (!e) {
-        AlignArgs a; a.F = num_frames; a.use_wheel = wheel_data ? 1 : 0; a.R = w.R; a.T = w.T; a.imu = w.imu; a.wheel = wheel_data ? w.wheel : nullptr;
-        memcpy(a.tic, tic, 24); a.g_norm = g_norm;
-        for (int k = 0; k < 9; k++) a.rio[k] = rio ? rio[k] : (k % 4 == 0 ? 1.0 : 0.0);
-        for (int k = 0; k < 3; k++) a.tio[k] = tio ? tio[k] : 0.0;
-        a.A = w.A; a.b = w.b; a.x = w.x; a.perm = w.perm; a.out = w.out;
-#ifdef VIWB_HOST_EMU
-        align_block(a, 0, 1);
-#else
-        g_prof.begin("align", ctx->stream); align_kernel<<<1, 128, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
-#endif
-        ctx->launches++;
-        e = dev_d2h(out.data(), w.out, (size_t)(n + 5) * 8, ctx->stream);
-    }
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(w.d);
-    if (e) return fail(ctx, VIWB_ERR_CUDA, "linear_alignment failed");
+    const int F = num_frames, n = 3 * F + 4;
+    std::vector<double> out((size_t)n + 5);
+    AlignArgs a; a.F = F; a.use_wheel = wheel_data ? 1 : 0;
+    memcpy(a.tic, tic, 24); a.g_norm = g_norm;
+    for (int k = 0; k < 9; k++) a.rio[k] = rio ? rio[k] : (k % 4 == 0 ? 1.0 : 0.0);
+    for (int k = 0; k < 3; k++) a.tio[k] = tio ? tio[k] : 0.0;
+    const int rc = staged(ctx, "linear_alignment", {stage_in(a.R, R, (size_t)F * 72), stage_in(a.T, T, (size_t)F * 24), stage_in(a.imu, imu_data, (size_t)(F - 1) * VIWB_IMU_DOUBLES * 8),
+                                                    stage_in(a.wheel, wheel_data, (size_t)(F - 1) * VIWB_WHEEL_DOUBLES * 8), stage_tmp(a.A, (size_t)2 * n * n * 8), stage_tmp(a.b, (size_t)(n + 8) * 8),
+                                                    stage_tmp(a.x, (size_t)(n + 8) * 8), stage_tmp(a.perm, (size_t)n * 4), stage_out(a.out, out.data(), out.size() * 8)}, [&] {
+        KERNEL(ctx, "align", 1, 1, 128, 0, align_kernel, (a), align_block(a, 0, 1));
+    });
+    if (rc) return rc;
     *aligned = out[0] != 0.0; memcpy(g, out.data() + 1, 24); *x_size = (int32_t)out[4];
     memcpy(x, out.data() + 5, (size_t)*x_size * 8);
     return VIWB_OK;
@@ -1463,59 +1416,21 @@ extern "C" int viwb_triangulate(viwb_context *ctx, const double *state, int n, c
     if (!ctx || !state || n < 0 || !stereo || !frame || !pt0 || !pt1 || !depth) return VIWB_ERR_INVALID;
     if (n == 0) return VIWB_OK;
     for (int k = 0; k < n; k++) if (frame[k] < 0 || frame[k] + (stereo[k] ? 0 : 1) > VIWB_WINDOW_SIZE) return fail(ctx, VIWB_ERR_INVALID, "triangulate: frame index out of the window");
-    bind_device(ctx);
-    const size_t bytes = align_up(SFIX * 8) + 2 * align_up((size_t)n * 4) + 2 * align_up((size_t)n * 16) + align_up((size_t)n * 8);
-    char *d = nullptr; CK(dev_malloc((void **)&d, bytes));
-    size_t o = 0;
-    double *d_x = (double *)(d + o); o += align_up(SFIX * 8);
-    int *d_st = (int *)(d + o); o += align_up((size_t)n * 4);
-    int *d_fr = (int *)(d + o); o += align_up((size_t)n * 4);
-    double *d_p0 = (double *)(d + o); o += align_up((size_t)n * 16);
-    double *d_p1 = (double *)(d + o); o += align_up((size_t)n * 16);
-    double *d_out = (double *)(d + o);
-    int e = dev_h2d(d_x, state, SFIX * 8, ctx->stream);
-    if (!e) e = dev_h2d(d_st, stereo, (size_t)n * 4, ctx->stream);
-    if (!e) e = dev_h2d(d_fr, frame, (size_t)n * 4, ctx->stream);
-    if (!e) e = dev_h2d(d_p0, pt0, (size_t)n * 16, ctx->stream);
-    if (!e) e = dev_h2d(d_p1, pt1, (size_t)n * 16, ctx->stream);
-    TriArgs a; a.n = n; a.state = d_x; a.stereo = d_st; a.frame = d_fr; a.pt0 = d_p0; a.pt1 = d_p1; a.init_depth = init_depth; a.depth = d_out;
-    if (!e) {
-#ifdef VIWB_HOST_EMU
-        for (int k = 0; k < n; k++) triangulate_item(a, k);
-#else
-        g_prof.begin("triangulate", ctx->stream); triangulate_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
-#endif
-        ctx->launches++;
-        e = dev_d2h(depth, d_out, (size_t)n * 8, ctx->stream);
-    }
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(d);
-    return e ? fail(ctx, VIWB_ERR_CUDA, "triangulate failed") : VIWB_OK;
+    TriArgs a; a.n = n; a.init_depth = init_depth;
+    return staged(ctx, "triangulate", {stage_in(a.state, state, SFIX * 8), stage_in(a.stereo, stereo, (size_t)n * 4), stage_in(a.frame, frame, (size_t)n * 4),
+                                       stage_in(a.pt0, pt0, (size_t)n * 16), stage_in(a.pt1, pt1, (size_t)n * 16), stage_out(a.depth, depth, (size_t)n * 8)}, [&] {
+        KERNEL(ctx, "triangulate", (n + 127) / 128, 1, 128, 0, triangulate_kernel, (a), for (int k = 0; k < n; k++) triangulate_item(a, k));
+    });
 }
 extern "C" int viwb_shift_depth(viwb_context *ctx, int n, const double *uv, const double *depth_in, const double *marg_R, const double *marg_P,
                                 const double *new_R, const double *new_P, double init_depth, double *depth_out) {
     if (!ctx || n < 0 || !uv || !depth_in || !marg_R || !marg_P || !new_R || !new_P || !depth_out) return VIWB_ERR_INVALID;
     if (n == 0) return VIWB_OK;
-    bind_device(ctx);
-    const size_t bytes = align_up((size_t)n * 24) + 2 * align_up((size_t)n * 8);
-    char *d = nullptr; CK(dev_malloc((void **)&d, bytes));
-    double *d_uv = (double *)d, *d_in = (double *)(d + align_up((size_t)n * 24)), *d_out = (double *)(d + align_up((size_t)n * 24) + align_up((size_t)n * 8));
-    int e = dev_h2d(d_uv, uv, (size_t)n * 24, ctx->stream);
-    if (!e) e = dev_h2d(d_in, depth_in, (size_t)n * 8, ctx->stream);
-    ShiftArgs a; a.n = n; a.uv = d_uv; a.depth_in = d_in; a.depth_out = d_out; a.init_depth = init_depth;
+    ShiftArgs a; a.n = n; a.init_depth = init_depth;
     memcpy(a.margR, marg_R, 72); memcpy(a.margP, marg_P, 24); memcpy(a.newR, new_R, 72); memcpy(a.newP, new_P, 24);
-    if (!e) {
-#ifdef VIWB_HOST_EMU
-        for (int k = 0; k < n; k++) shift_depth_item(a, k);
-#else
-        g_prof.begin("shift_depth", ctx->stream); shift_depth_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
-#endif
-        ctx->launches++;
-        e = dev_d2h(depth_out, d_out, (size_t)n * 8, ctx->stream);
-    }
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(d);
-    return e ? fail(ctx, VIWB_ERR_CUDA, "shift_depth failed") : VIWB_OK;
+    return staged(ctx, "shift_depth", {stage_in(a.uv, uv, (size_t)n * 24), stage_in(a.depth_in, depth_in, (size_t)n * 8), stage_out(a.depth_out, depth_out, (size_t)n * 8)}, [&] {
+        KERNEL(ctx, "shift_depth", (n + 127) / 128, 1, 128, 0, shift_depth_kernel, (a), for (int k = 0; k < n; k++) shift_depth_item(a, k));
+    });
 }
 // Estimator::predictPtsInNextFrame (estimator.cpp:2080-2113): thread per feature of the caller's FeatureManager::feature list
 extern "C" int viwb_predict_pts(viwb_context *ctx, const double *state, int frame_count, int n, const int32_t *start_frame, const int32_t *num_obs, const double *pt0,
@@ -1524,36 +1439,12 @@ extern "C" int viwb_predict_pts(viwb_context *ctx, const double *state, int fram
     if (frame_count < 0 || frame_count > VIWB_WINDOW_SIZE) return fail(ctx, VIWB_ERR_INVALID, "predict_pts: frame_count out of the window");
     for (int k = 0; k < n; k++) if (start_frame[k] < 0 || start_frame[k] > VIWB_WINDOW_SIZE || num_obs[k] < 0) return fail(ctx, VIWB_ERR_INVALID, "predict_pts: start_frame out of the window or negative num_obs");
     if (n == 0) return VIWB_OK;
-    bind_device(ctx);
-    const size_t bytes = align_up(SFIX * 8) + 2 * align_up((size_t)n * 4) + 2 * align_up((size_t)n * 24) + align_up((size_t)n * 8) + align_up((size_t)n);
-    char *d = nullptr; CK(dev_malloc((void **)&d, bytes));
-    size_t o = 0;
-    double *d_x = (double *)(d + o); o += align_up(SFIX * 8);
-    int *d_sf = (int *)(d + o); o += align_up((size_t)n * 4);
-    int *d_no = (int *)(d + o); o += align_up((size_t)n * 4);
-    double *d_p0 = (double *)(d + o); o += align_up((size_t)n * 24);
-    double *d_out = (double *)(d + o); o += align_up((size_t)n * 24);
-    double *d_dep = (double *)(d + o); o += align_up((size_t)n * 8);
-    uint8_t *d_val = (uint8_t *)(d + o);
-    int e = dev_h2d(d_x, state, SFIX * 8, ctx->stream);
-    if (!e) e = dev_h2d(d_sf, start_frame, (size_t)n * 4, ctx->stream);
-    if (!e) e = dev_h2d(d_no, num_obs, (size_t)n * 4, ctx->stream);
-    if (!e) e = dev_h2d(d_p0, pt0, (size_t)n * 24, ctx->stream);
-    if (!e) e = dev_h2d(d_dep, depth, (size_t)n * 8, ctx->stream);
-    PredictArgs a; a.n = n; a.frame_count = frame_count; a.state = d_x; a.start_frame = d_sf; a.num_obs = d_no; a.pt0 = d_p0; a.depth = d_dep; a.pts_cam = d_out; a.valid = d_val;
-    if (!e) {
-#ifdef VIWB_HOST_EMU
-        for (int k = 0; k < n; k++) predict_pts_item(a, k);
-#else
-        g_prof.begin("predict_pts", ctx->stream); predict_pts_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
-#endif
-        ctx->launches++;
-        e = dev_d2h(pts_cam, d_out, (size_t)n * 24, ctx->stream);
-        if (!e) e = dev_d2h(valid, d_val, (size_t)n, ctx->stream);
-    }
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(d);
-    return e ? fail(ctx, VIWB_ERR_CUDA, "predict_pts failed") : VIWB_OK;
+    PredictArgs a; a.n = n; a.frame_count = frame_count;
+    return staged(ctx, "predict_pts", {stage_in(a.state, state, SFIX * 8), stage_in(a.start_frame, start_frame, (size_t)n * 4), stage_in(a.num_obs, num_obs, (size_t)n * 4),
+                                       stage_in(a.pt0, pt0, (size_t)n * 24), stage_in(a.depth, depth, (size_t)n * 8), stage_out(a.pts_cam, pts_cam, (size_t)n * 24),
+                                       stage_out(a.valid, valid, (size_t)n)}, [&] {
+        KERNEL(ctx, "predict_pts", (n + 127) / 128, 1, 128, 0, predict_pts_kernel, (a), for (int k = 0; k < n; k++) predict_pts_item(a, k));
+    });
 }
 
 extern "C" int viwb_undistort_velocity(viwb_context *ctx, const viwb_pinhole *cam, int n, const float *pts, const float *prev_un_pts, const uint8_t *has_prev,
@@ -1569,30 +1460,12 @@ extern "C" int viwb_undistort_velocity_camera(viwb_context *ctx, const viwb_came
     CamModel cm;
     if (camera_model(ctx, cam, &cm)) return VIWB_ERR_INVALID;
     if (n == 0) return VIWB_OK;
-    bind_device(ctx);
-    const size_t pb = align_up((size_t)n * 8);
-    char *d = nullptr; CK(dev_malloc((void **)&d, 4 * pb + align_up((size_t)n)));
-    float *d_pts = (float *)d, *d_prev = (float *)(d + pb), *d_un = (float *)(d + 2 * pb), *d_vel = (float *)(d + 3 * pb);
-    unsigned char *d_hp = (unsigned char *)(d + 4 * pb);
-    int e = dev_h2d(d_pts, pts, (size_t)n * 8, ctx->stream);
-    if (!e && prev_un_pts) e = dev_h2d(d_prev, prev_un_pts, (size_t)n * 8, ctx->stream);
-    if (!e && has_prev) e = dev_h2d(d_hp, has_prev, (size_t)n, ctx->stream);
-    UndistArgs a; a.n = n; a.pts = d_pts; a.prev_un = prev_un_pts ? d_prev : nullptr; a.has_prev = has_prev ? d_hp : nullptr;
+    UndistArgs a; a.n = n;
     a.fx = cm.fx; a.fy = cm.fy; a.cx = cm.cx; a.cy = cm.cy; a.k1 = cm.k1; a.k2 = cm.k2; a.p1 = cm.p1; a.p2 = cm.p2; a.dt = dt; a.model = cm.model; a.xi = cm.xi;
-    a.un = d_un; a.vel = velocity ? d_vel : nullptr;
-    if (!e) {
-#ifdef VIWB_HOST_EMU
-        for (int k = 0; k < n; k++) undistort_item(a, k);
-#else
-        g_prof.begin("undistort", ctx->stream); undistort_kernel<<<(n + 127) / 128, 128, 0, ctx->stream>>>(a); g_prof.end(ctx->stream);
-#endif
-        ctx->launches++;
-        e = dev_d2h(un_pts, d_un, (size_t)n * 8, ctx->stream);
-        if (!e && velocity) e = dev_d2h(velocity, d_vel, (size_t)n * 8, ctx->stream);
-    }
-    if (!e) e = dev_sync(ctx->stream);
-    dev_free(d);
-    return e ? fail(ctx, VIWB_ERR_CUDA, "undistort failed") : VIWB_OK;
+    return staged(ctx, "undistort", {stage_in(a.pts, pts, (size_t)n * 8), stage_in(a.prev_un, prev_un_pts, (size_t)n * 8), stage_in(a.has_prev, has_prev, (size_t)n),
+                                     stage_out(a.un, un_pts, (size_t)n * 8), stage_out(a.vel, velocity, (size_t)n * 8)}, [&] {
+        KERNEL(ctx, "undistort", (n + 127) / 128, 1, 128, 0, undistort_kernel, (a), for (int k = 0; k < n; k++) undistort_item(a, k));
+    });
 }
 
 // -------------------------------------------------------------------------------------- feature tracker
