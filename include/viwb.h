@@ -368,14 +368,26 @@ int viwb_undistort_velocity(viwb_context *ctx, const viwb_pinhole *cam, int n, c
  *   VIWB_CAMERA_MEI:     p = xi k1 k2 p1 p2 gamma1 gamma2 u0 v0 (CataCamera's constructor and its yaml order, CataCamera.cc:300-303), the
  *                        unified omnidirectional model with mirror parameter xi: the lift is CataCamera::liftProjective (:556-626, recursive
  *                        distortion n = 8, distortion :766-782, m_inv_K* :319-323) and the projection CataCamera::spaceToPlane (:636-659).
- * The MEI arithmetic is rounded operation by operation (no fused multiply-add), so its floats are the reference's bit for bit.  Parameter
- * values are not checked, as the reference does not check them: a ray with 1 + (1 - xi^2) rho^2 < 0 lifts to NaN as it does there. */
-typedef enum { VIWB_CAMERA_PINHOLE = 0, VIWB_CAMERA_MEI = 1 } viwb_camera_model;
+ *   VIWB_CAMERA_KANNALA_BRANDT: p = k2 k3 k4 k5 mu mv u0 v0 (EquidistantCamera::Parameters' and its yaml order; p[8] unused), the
+ *                        generic fisheye model r(theta) = theta + k2 theta^3 + k3 theta^5 + k4 theta^7 + k5 theta^9 (Kalibr's `equidistant`,
+ *                        OpenCV's cv::fisheye): the lift is EquidistantCamera::liftProjective (:428-442, m_inv_K* :271-274) over
+ *                        backprojectSymmetric (:716-818: theta = the smallest non-negative real root of r(theta) = |p_u|, from the eigenvalues
+ *                        of the polynomial's companion matrix, restated from Eigen 3.3's EigenSolver), the projection
+ *                        EquidistantCamera::spaceToPlane (:451-461, r() of EquidistantCamera.h:158-168).
+ * The MEI arithmetic is rounded operation by operation (no fused multiply-add), so its floats are the reference's bit for bit.  So is the
+ * Kannala-Brandt arithmetic, except for sin / cos / acos / atan2, which the GPU evaluates within 2 ulp: a float may then differ from the
+ * reference's by one ulp where the double lies next to a float rounding boundary.  Parameter values are not checked, as the reference does
+ * not check them: a ray with 1 + (1 - xi^2) rho^2 < 0 lifts to NaN as it does there, a Kannala-Brandt ray past 90 degrees lifts to the
+ * mirrored point.  The one refusal: a Kannala-Brandt camera whose companion matrix would divide by zero is VIWB_ERR_INVALID.  That is the
+ * case where the polynomial degree npow (9, less 2 for every k_i == 0, wherever it sits) is above 1 and its coefficient at npow is 0 --
+ * k4 == 0 with k5 != 0, or k2 == k4 == k5 == 0 with k3 != 0, for example; the reference then feeds inf / NaN to its eigen-solver. */
+typedef enum { VIWB_CAMERA_PINHOLE = 0, VIWB_CAMERA_MEI = 1, VIWB_CAMERA_KANNALA_BRANDT = 2 } viwb_camera_model;
 typedef struct viwb_camera {
     int32_t model;      /* viwb_camera_model */
     double p[9];
 } viwb_camera;
-/* viwb_undistort_velocity with the lift of `cam`'s model.  An unknown model or a NULL cam is VIWB_ERR_INVALID (viwb_last_error says why).
+/* viwb_undistort_velocity with the lift of `cam`'s model.  An unknown model, a NULL cam or a refused Kannala-Brandt camera is
+ * VIWB_ERR_INVALID (viwb_last_error says why).
  * With a PINHOLE camera this is viwb_undistort_velocity, to the bit. */
 int viwb_undistort_velocity_camera(viwb_context *ctx, const viwb_camera *cam, int n, const float *pts, const float *prev_un_pts,
                                    const uint8_t *has_prev, double dt, float *un_pts, float *velocity);
@@ -456,7 +468,8 @@ int viwb_tracker_create(viwb_context *ctx, int streams, int width, int height, c
 /* viwb_tracker_create with cam[0] / cam[1] = m_camera[0] / m_camera[1] of any viwb_camera model, each camera its own (an MEI left camera
  * beside a pinhole right camera is legal); config->cam is not read.  Both entries must name a known model, cam[1] also in a mono session,
  * where it is not used.  The lift of undistortedPts (feature_tracker.cpp:606-617, both cameras) and setPrediction's spaceToPlane
- * (:729, camera 0, viwb_tracker_feedback) follow each camera's model.  An unknown model or a NULL cam is VIWB_ERR_INVALID. */
+ * (:729, camera 0, viwb_tracker_feedback) follow each camera's model.  An unknown model, a NULL cam or a refused Kannala-Brandt camera
+ * is VIWB_ERR_INVALID, and no session is made. */
 int viwb_tracker_create_camera(viwb_context *ctx, int streams, int width, int height, const viwb_tracker_config *config,
                                const viwb_camera cam[2], viwb_tracker **out);
 void viwb_tracker_destroy(viwb_tracker *t);
@@ -475,7 +488,7 @@ int viwb_tracker_download(viwb_tracker *t, int32_t *n_left, int32_t *ids, int32_
  * FeatureTracker::removeOutliers(remove_ids) (feature_tracker.cpp:739-755: stable reduceVector of prev_pts, ids, track_cnt; the id ->
  * undistorted point maps stay as they are) and then, for the streams with has_prediction[s] != 0, FeatureTracker::setPrediction
  * (:715-736): for each remaining row, the prediction with the row's id projected by m_camera[0]->spaceToPlane (pinhole + radtan,
- * PinholeCamera.cc:520-542, or MEI, CataCamera.cc:636-659) and rounded to float as cv::Point2f does, else the row's prev_pts.  The prediction stays in HBM and is
+ * PinholeCamera.cc:520-542, MEI, CataCamera.cc:636-659, or Kannala-Brandt, EquidistantCamera.cc:451-461) and rounded to float as cv::Point2f does, else the row's prev_pts.  The prediction stays in HBM and is
  * consumed by the next viwb_tracker_track, which must then be called with predict_pts == NULL (VIWB_ERR_INVALID otherwise, and the
  * session stays as it was); hasPrediction is cleared by that tick (:279).
  * n_remove / n_pred: [streams] list lengths; remove_ids, pred_ids: the streams' lists back to back; pred_pts_cam: [sum n_pred][3]

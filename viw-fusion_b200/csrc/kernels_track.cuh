@@ -17,7 +17,7 @@
 
 namespace viwb {
 
-typedef CamModel TrkCam;                 // m_camera[0] / m_camera[1]: PINHOLE or MEI (kernels_feat.cuh)
+typedef CamModel TrkCam;                 // m_camera[0] / m_camera[1]: PINHOLE, MEI or KANNALA_BRANDT (kernels_feat.cuh)
 
 struct TrkArgs {                         // one camera stream; every array holds `maxn` entries
     // --- tracker buffers (viwb_lk_batch): prev_pts = points of the previous image, lk_cur = temporal LK result, stereo_in / right = stereo LK in / out
@@ -50,7 +50,8 @@ VIWB_D int trk_rank(bool flag, int tid, int &total) {
 #endif
 }
 
-// PinholeCamera::liftProjective (camera_models/src/camera_models/PinholeCamera.cc:450-517) or CataCamera::liftProjective (CataCamera.cc:556-626)
+// PinholeCamera::liftProjective (camera_models/src/camera_models/PinholeCamera.cc:450-517), CataCamera::liftProjective (CataCamera.cc:556-626)
+// or EquidistantCamera::liftProjective (EquidistantCamera.cc:428-442)
 // narrowed to cv::Point2f (feature_tracker.cpp:614)
 VIWB_D void trk_lift(const TrkCam &c, float u, float v, float &x, float &y) {
     UndistArgs a; a.n = 1; a.pts = nullptr; a.prev_un = nullptr; a.has_prev = nullptr; a.vel = nullptr;
@@ -104,9 +105,11 @@ VIWB_D int trk_find_id(const int *ids, int n, int id) {          // position of 
 }
 // PinholeCamera::spaceToPlane (PinholeCamera.cc:520-542, distortion :646-662) narrowed to cv::Point2f (feature_tracker.cpp:730).  Every
 // product and sum is rounded on its own (no fused multiply-add), so that the pixel is the float the reference's build (-ffp-contract=off
-// here, SSE2 there) hands to calcOpticalFlowPyrLK, bit for bit.  An MEI camera projects through CataCamera::spaceToPlane instead.
+// here, SSE2 there) hands to calcOpticalFlowPyrLK, bit for bit.  An MEI camera projects through CataCamera::spaceToPlane instead,
+// a Kannala-Brandt one through EquidistantCamera::spaceToPlane (kb_space_to_plane).
 VIWB_D void trk_space_to_plane(const TrkCam &c, const double *P, float &u, float &v) {
     if (c.model == CAM_MEI) { mei_space_to_plane(c, P, u, v); return; }
+    if (c.model == CAM_KB) { kb_space_to_plane(c, P, u, v); return; }
     const double x = P[0] / P[2], y = P[1] / P[2];
     double xd = x, yd = y;
     if (!(c.k1 == 0.0 && c.k2 == 0.0 && c.p1 == 0.0 && c.p2 == 0.0)) {       // m_noDistortion

@@ -405,12 +405,12 @@ class Context:
         self._ck(self.lib.viwb_host_unregister(self.h, C.c_void_p(arr.ctypes.data)), "viwb_host_unregister")
 
 
-CAMERA_PINHOLE, CAMERA_MEI = 0, 1
+CAMERA_PINHOLE, CAMERA_MEI, CAMERA_KANNALA_BRANDT = 0, 1, 2
 MAX_LANDMARKS = 1000          # VIWB_MAX_LANDMARKS, the per-stream landmark stride of the viwb_features_* arrays
 
 
 class Camera(C.Structure):
-    """viwb_camera: a camera of either model (include/viwb.h).  Build one with Camera.pinhole(...) or Camera.mei(...)."""
+    """viwb_camera: a camera of any model (include/viwb.h).  Build one with Camera.pinhole(...), Camera.mei(...) or Camera.kannala_brandt(...)."""
     _fields_ = [("model", C.c_int32), ("p", C.c_double * 9)]
 
     @classmethod
@@ -421,6 +421,12 @@ class Camera(C.Structure):
     def mei(cls, xi, k1, k2, p1, p2, gamma1, gamma2, u0, v0):
         """the parameters in the order of a camodocal MEI yaml file (CataCamera's constructor)"""
         return cls(CAMERA_MEI, (C.c_double * 9)(xi, k1, k2, p1, p2, gamma1, gamma2, u0, v0))
+
+    @classmethod
+    def kannala_brandt(cls, k2, k3, k4, k5, mu, mv, u0, v0):
+        """the parameters in the order of a camodocal KANNALA_BRANDT yaml file (EquidistantCamera::Parameters); Kalibr's `equidistant`
+        intrinsics (fu, fv, pu, pv) and distortion (k1..k4) are mu, mv, u0, v0 and k2..k5"""
+        return cls(CAMERA_KANNALA_BRANDT, (C.c_double * 9)(k2, k3, k4, k5, mu, mv, u0, v0, 0.0))
 
 
 class TrackerConfig(C.Structure):
