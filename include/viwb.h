@@ -301,6 +301,10 @@ int viwb_batch_download(viwb_context *ctx, viwb_batch *b, double *const *states,
 int viwb_batch_outliers(viwb_context *ctx, viwb_batch *b, double focal_length, double threshold_px, uint8_t *const *outliers);
 /* algorithmic bytes of one viwb_batch_run (SURVEY 8(d) B_solve model, summed over the batch) */
 double viwb_batch_algorithmic_bytes(const viwb_batch *b);
+/* The solve kernel's launch for this batch: threads per block, dynamic shared memory per block (bytes; sized by the batch's widest window) and
+ * how many such blocks one SM of the context's device holds (cudaOccupancyMaxActiveBlocksPerMultiprocessor).  Measurement only, like
+ * viwb_launch_count.  Any output pointer may be NULL. */
+int viwb_batch_solve_launch(viwb_context *ctx, const viwb_batch *b, int *threads, int *smem_bytes, int *blocks_per_sm);
 void viwb_batch_destroy(viwb_context *ctx, viwb_batch *b);
 
 /* Normal equations at `state` exactly as the solver assembles them (debug/parity hook):

@@ -105,7 +105,7 @@ VIWB_D void asm_items_block(const BatchDev &bd, int bx, int by, int tid, int nt,
 //                     void add(int i, int j, double v)  for an unordered index pair (called once per pair per phase),
 //                     void addg(int i, double v).
 struct PackedTarget {      // solver: skyline lower triangle in shared memory over the compact active columns
-    double *L, *g; const short *tcol; const int *rp, *fst;
+    double *L, *g; const short *tcol; const short *rp, *fst;
     VIWB_DM int col(int blk, int k) const { return (tcol[blk] >= 0 && k < blk_tsize(blk)) ? tcol[blk] + k : -1; }
     VIWB_DM void add(int i, int j, double v) const { if (i < j) { const int t = i; i = j; j = t; } L[rp[i] - fst[i] + j] += v; }
     VIWB_DM void addg(int i, double v) const { g[i] += v; }

@@ -7,8 +7,8 @@
 //
 // The reduced system (<= 192 active tangent columns) lives in shared memory as a SKYLINE: row i of the lower triangle is stored
 // from its first structurally non-zero column efirst[i] (host symbolic analysis, csrc/viwb.cu lower_count).  With the speed-bias
-// blocks eliminated first, newest frame first, the stereo+IMU window needs 7.2 K instead of 13.7 K doubles, which lets two
-// windows share an SM.  All quadratic forms are evaluated on the *unscaled* matrices with unscaled directions
+// blocks eliminated first, newest frame first, the stereo+IMU window needs 7.2-7.6 K instead of 13.7 K doubles; with the carve below
+// (9.5 K doubles at 256 threads) three such windows share an SM.  All quadratic forms are evaluated on the *unscaled* matrices with unscaled directions
 // u = c o (v / D), which equals Ceres' J_scaled products exactly.
 #pragma once
 #include <vector>
@@ -62,25 +62,95 @@ VIWB_D void block_sum_n(double (&v)[N], int tid, int nt, double *red) {
 #endif
 }
 
+// The solve kernel's sums are stated over a fixed VIRTUAL layout of SOLVE_VNT threads (12 warps), whatever the block's real size: real thread t
+// owns the virtual threads t, t + nt, ... below SOLVE_VNT (SOLVE_VPT of them at most), keeps one partial sum per virtual thread, strides its loops
+// by SOLVE_VNT and reduces each virtual warp with the same shuffle tree; the virtual warps' slots are then added in order.  So every sum is the
+// same double at any block size that is a multiple of 32, and the block size only changes the occupancy.  (Maxima need no such care: fmax does
+// not depend on the order.)  The emulation runs one thread per block, and its virtual layout is that thread.
+#ifndef SOLVE_NT
+#define SOLVE_NT 256
+#endif
+#ifdef VIWB_HOST_EMU
+enum { SOLVE_VNT = 1, SOLVE_VW = 1, SOLVE_VPT = 1 };
+#define VIWB_VT_LOOP(j, vt) for (int j = 0, vt = tid; j < SOLVE_VPT; j++, vt += nt)
+#define VIWB_VLM_LOOP(k, vt, N) for (int k = (vt), lane = 0; k < (N); k++)
+#else
+enum { SOLVE_VNT = 384, SOLVE_VW = SOLVE_VNT / 32, SOLVE_VPT = (SOLVE_VNT + SOLVE_NT - 1) / SOLVE_NT };
+#define VIWB_VT_LOOP(j, vt) _Pragma("unroll") for (int j = 0, vt = tid; j < SOLVE_VPT; j++, vt += nt) if (vt < SOLVE_VNT)
+// one virtual warp per landmark (vt >> 5 is warp-uniform): lane 0 carries the scalar work and the virtual thread's partial sums
+#define VIWB_VLM_LOOP(k, vt, N) for (int k = (vt) >> 5, lane = tid & 31; k < (N); k += SOLVE_VW)
+#endif
+// v[j][q]: partial sum q of this thread's virtual thread j (0 where it owns none); on return every thread has the block's sums in v[0][q].
+// red needs N * SOLVE_RED doubles.
+enum { SOLVE_RED = 16 };      // slots per sum: >= the virtual warps and the real ones (block_max)
+template <int N>
+VIWB_D void vblock_sum_n(double (&v)[SOLVE_VPT][N], int tid, int nt, double *red) {
+#ifdef VIWB_HOST_EMU
+    (void)v; (void)tid; (void)nt; (void)red;
+#else
+#pragma unroll
+    for (int j = 0; j < SOLVE_VPT; j++) {
+        const int vt = tid + j * nt;
+        if (vt < SOLVE_VNT) {
+#pragma unroll
+            for (int q = 0; q < N; q++) for (int o = 16; o > 0; o >>= 1) v[j][q] += __shfl_down_sync(0xffffffffu, v[j][q], o);
+            if ((tid & 31) == 0) for (int q = 0; q < N; q++) red[q * SOLVE_RED + (vt >> 5)] = v[j][q];
+        }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int q = 0; q < N; q++) { double r = 0.0; for (int k = 0; k < SOLVE_VW; k++) r += red[q * SOLVE_RED + k]; v[0][q] = r; }
+    __syncthreads();
+#endif
+}
+
+// Shared memory of one window, in doubles.  P = solve_nfp(nf_max): the batch's largest nf in whole 4-double groups; R = solve_panel_rows(nf_max):
+// the most trailing rows (rhs included, whole 4-row tiles) a panel has, the first panel's; F = solve_fac_warps(nt, nf_max): the warps that hold
+// such rows and factor the diagonal block.
+//   L     skyline lower triangle, env_max entries (even).  The factor's diagonal holds the inverse pivots 1 / L_kk, which is all the
+//         back-substitution reads there.
+//   U     union region, max(8 R + CHOL_SCR F, 2 P + 2 VSUB); its parts are live at different times of a step:
+//           U[0, P)               g (assembly) | ug (Cauchy point) | u (back-substituted step -> quadratic forms)
+//           U[P, 2 P)             imap (assembly, ints) | Hu (Cauchy point, quadratic forms) | xo (back-substitution)
+//           U[2 P, 2 P + 2 VSUB)  uvis (Cauchy point, landmark back-substitution)
+//           U[0, 8 R)             Pt (Cholesky; 16-byte aligned), then chol: CHOL_SCR per factoring warp (Cholesky)
+//         The assembled gradient is read from its copy in HBM (gpk) after the assembly, and the Jacobi scales, D and the scaled gradient from
+//         the window's v_* slices, where they are written once per linearisation; the forms recompute ug from those.
+//   y     P: right-hand side, then solution of the reduced system (the Cholesky's row n, addressed from L)
+//   red   5 * SOLVE_RED: reductions
+//   then shorts: vmap (P), fst (P), rp (P + 1)
 struct SolveSmem {
-    double *L;       // skyline lower triangle: row i holds columns fst[i]..i at L[rp[i] .. rp[i+1])
-    int *rp, *fst;   // row pointers (nf + 1) and first columns (nf)
-    double *g, *sc, *D, *sg, *y, *u, *Hu, *ug, *uvis, *red, *bc, *chol, *dinv, *xo, *Pt;
-    int *amap, *vmap;
+    double *L;            // skyline lower triangle: row i holds columns fst[i]..i at L[rp[i] .. rp[i+1])
+    short *rp, *fst;      // row pointers (nf + 1) and first columns (nf)
+    short *vmap;          // compact column -> visual subspace (-1: not visual)
+    double *g, *ug, *u, *Hu, *xo, *Pt, *uvis, *chol, *y, *red;
+    int ldp;              // row stride of Pt (R)
 };
-VIWB_HD size_t solve_smem_doubles(int nt, int esize) { return (size_t)((esize + 1) & ~1) + 9 * TFIX + 2 * VSUB + 5 * 32 + 16 + 2 * TFIX + 2 + (size_t)((nt + 31) / 32) * 48 + 2 * TFIX + 8 * (TFIX + 4) + 2 * TFIX + 2; }   // ints: amap, vmap, rp, fst
-VIWB_D void carve(SolveSmem &s, double *smem, int nt, int esize) {
+enum { CHOL_NB = 8, CHOL_SCR = 48 };      // the Cholesky's panel width and per-warp scratch (doubles)
+VIWB_HD int solve_nfp(int nf_max) { const int p = (nf_max + 3) & ~3; return p > 4 ? p : 4; }
+VIWB_HD int solve_panel_rows(int nf_max) { const int r = nf_max > CHOL_NB ? (nf_max + 1 - CHOL_NB + 3) & ~3 : 4; return r; }
+VIWB_HD int solve_fac_warps(int nt, int nf_max) { const int a = (nt + 31) / 32, b = (solve_panel_rows(nf_max) + 31) / 32; return a < b ? a : b; }
+VIWB_HD size_t solve_union_doubles(int nt, int nf_max) {
+    const size_t a = (size_t)8 * solve_panel_rows(nf_max) + (size_t)CHOL_SCR * solve_fac_warps(nt, nf_max), b = (size_t)2 * solve_nfp(nf_max) + 2 * VSUB;
+    return a > b ? a : b;
+}
+VIWB_HD size_t solve_smem_doubles(int nt, int esize, int nf_max) {
+    const int P = solve_nfp(nf_max);
+    return (size_t)((esize + 1) & ~1) + solve_union_doubles(nt, nf_max) + P + 5 * SOLVE_RED + (size_t)(3 * P + 1 + 3) / 4;
+}
+VIWB_HD void carve(SolveSmem &s, double *smem, int nt, int esize, int nf_max) {
+    const int P = solve_nfp(nf_max), R = solve_panel_rows(nf_max);
     double *p = smem;
     s.L = p; p += (size_t)((esize + 1) & ~1);
-    s.g = p; p += TFIX; s.sc = p; p += TFIX; s.D = p; p += TFIX; s.sg = p; p += TFIX; s.y = p; p += TFIX;
-    s.u = p; p += TFIX; s.Hu = p; p += TFIX; s.ug = p; p += TFIX;
-    s.uvis = p; p += 2 * VSUB;
-    s.red = p; p += 5 * 32; s.bc = p; p += 16;
-    s.chol = p; p += (size_t)((nt + 31) / 32) * 48;
-    s.dinv = p; p += TFIX; s.xo = p; p += TFIX;
-    if ((p - smem) & 1) p++;                    // Pt is read with 16-byte vector loads
-    s.Pt = p; p += 8 * (TFIX + 4);
-    s.amap = (int *)p; s.vmap = s.amap + TFIX; s.rp = s.vmap + TFIX; s.fst = s.rp + TFIX + 2;
+    double *U = p; p += solve_union_doubles(nt, nf_max);
+    s.g = s.ug = s.u = U;
+    s.Hu = s.xo = U + P;
+    s.uvis = U + 2 * P;
+    s.Pt = U; s.ldp = R;
+    s.chol = U + 8 * R;
+    s.y = p; p += P;
+    s.red = p; p += 5 * SOLVE_RED;
+    s.vmap = (short *)p; s.fst = s.vmap + P; s.rp = s.fst + P;
 }
 // entry (i, j), j <= i, of the skyline; must lie inside the envelope
 #define SKY(s, i, j) ((s).L[(s).rp[i] - (s).fst[i] + (j)])
@@ -92,7 +162,7 @@ VIWB_D void assemble_H(const BatchDev &bd, int w, const SolveSmem &s, int nf, do
     for (int i = tid; i < nf; i += nt) s.g[i] = 0.0;
     VIWB_SYNC();
     PackedTarget t; t.L = s.L; t.g = s.g; t.tcol = bd.meta[w].tcol; t.rp = s.rp; t.fst = s.fst;
-    assemble_into(t, bd, w, MODE_SOLVE, tid, nt, (int *)s.Hu);      // Hu is free until the step computation
+    assemble_into(t, bd, w, MODE_SOLVE, tid, nt, (int *)s.Hu);      // Hu is free until the Cauchy point
     for (int e = tid; e < ne; e += nt) Hpk[e] = s.L[e];
     for (int i = tid; i < nf; i += nt) gpk[i] = s.g[i];
     VIWB_SYNC();
@@ -140,7 +210,7 @@ VIWB_D double warp_dot80(const double *W, const double *v, int lane) {
     return a;
 #endif
 }
-// landmark loops run one warp per landmark: lane 0 carries the scalar work and the partial sums
+// landmark loops that feed no sum run one real warp per landmark (lane 0 carries the scalar work)
 #ifdef VIWB_HOST_EMU
 #define VIWB_LM_LOOP(k, N) for (int k = 0, lane = 0; k < (N); k++)
 #else
@@ -155,8 +225,9 @@ VIWB_D double warp_dot80(const double *W, const double *v, int lane) {
 //   one thread per panel row, which also drops its 8 results into a column-major panel buffer Pt[8][rows]; the trailing
 //   update then runs 4x4 register tiles whose operands are 32-byte vector loads from Pt (conflict-free), not strided
 //   reads of the packed triangle.
-// scratch: nwarps * 48 doubles (36 packed block entries + 8 inverse pivots + flag); dinv[n] receives 1 / L_kk;
-// Pt: 8 * CHOL_LDP doubles, 16-byte aligned.
+// scratch: CHOL_SCR doubles per warp that holds panel rows (36 packed block entries + 8 inverse pivots + flag); on exit the diagonal of L holds the
+// inverse pivots 1 / L_kk instead of L_kk (the back-substitution multiplies by them, and nothing else reads the factor's diagonal);
+// Pt: 8 rows of ldp >= the panel rows rounded up to 4 (a multiple of 4) doubles, 16-byte aligned.
 VIWB_D void load4(const double *p, double *o) {
 #ifdef VIWB_HOST_EMU
     o[0] = p[0]; o[1] = p[1]; o[2] = p[2]; o[3] = p[3];
@@ -165,7 +236,6 @@ VIWB_D void load4(const double *p, double *o) {
     o[0] = a.x; o[1] = a.y; o[2] = b.x; o[3] = b.y;
 #endif
 }
-enum { CHOL_NB = 8, CHOL_SCR = 48, CHOL_LDP = TFIX + 4 };
 // Phase probe (measurement build only, `make phases` -> libviwb_phases.so): thread 0 reads clock64() at the barrier-delimited phase
 // boundaries of a launch that computes a step and adds the cycles since the previous boundary to its window's slot of the phase.
 // The sub-phases of the Cholesky and the back-substitution are summed in registers and written once per factorisation (SOLVE_FLUSH).
@@ -222,7 +292,7 @@ inline void chol_plan_build(const short *efirst, int n, std::vector<int> &plan) 
     }
     plan[n + 1 + np] = (int)plan.size() - head;
 }
-VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double *y, int n, int tid, int nt, double *scratch, double *dinv, double *Pt,
+VIWB_D bool cholesky_packed_rhs(double *L, const short *rp, const short *fst, double *y, int n, int tid, int nt, double *scratch, double *Pt, int ldp,
                                 const int *__restrict__ plan, SolveClock &sph) {
     (void)sph;
     const int yoff = (int)(y - L);
@@ -237,7 +307,7 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
         const int nb = (n - c0) < CHOL_NB ? (n - c0) : CHOL_NB;
         const int r0 = c0 + nb;
         const int nr = n + 1 - r0, mt = (nr + 3) / 4;       // panel rows r0..n (row n = rhs), padded to whole 4-row tiles
-        // only the warps that hold panel rows factor the diagonal block (warp 0 always: row n, dinv and the block's write-back); the others
+        // only the warps that hold panel rows factor the diagonal block (warp 0 always: row n and the block's write-back); the others
         // would only take issue slots from them
         const bool fac = (tid & ~31) < 4 * mt;
 #ifdef VIWB_HOST_EMU
@@ -314,14 +384,14 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
                 for (int k = 0; k < 8; k++) if (k < nb && c0 + k >= fi) ri[k] = x[k];
             }
 #pragma unroll
-            for (int k = 0; k < 8; k++) Pt[k * CHOL_LDP + (i - r0)] = x[k];
+            for (int k = 0; k < 8; k++) Pt[k * ldp + (i - r0)] = x[k];
         }
-        for (int r = tid; r < nb; r += nt) dinv[c0 + r] = my[36 + r];
         VIWB_SYNC();
         SOLVE_LAP(SPH_CHOL_PANEL);
         if (scratch[44] == 0.0) return false;               // warp 0's verdict, the same as every factoring warp's: every thread returns here
-        // factored diagonal block back into the matrix (only now: the other warps have finished reading the unfactored one)
-        for (int r = tid; r < nb; r += nt) { double *rk = ROW(c0 + r) + c0; const int fr = FST(c0 + r); for (int j = 0; j <= r; j++) if (c0 + j >= fr) rk[j] = my[r * (r + 1) / 2 + j]; }
+        // factored diagonal block back into the matrix (only now: the other warps have finished reading the unfactored one), inverse pivots on
+        // the diagonal
+        for (int r = tid; r < nb; r += nt) { double *rk = ROW(c0 + r) + c0; const int fr = FST(c0 + r); for (int j = 0; j <= r; j++) if (c0 + j >= fr) rk[j] = j == r ? my[36 + r] : my[r * (r + 1) / 2 + j]; }
         // trailing update with 4x4 register tiles over the plan's tiles of this panel: each receiving entry a_ik -= sum_m L_im L_km once
         for (int t = tid; t < ntp; t += nt) {
             const unsigned cur = wd;
@@ -335,7 +405,7 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
 #pragma unroll
             for (int m = 0; m < 8; m++) {
                 double li[4], lk[4];
-                load4(Pt + m * CHOL_LDP + 4 * ti, li); load4(Pt + m * CHOL_LDP + 4 * tk, lk);
+                load4(Pt + m * ldp + 4 * ti, li); load4(Pt + m * ldp + 4 * tk, lk);
 #pragma unroll
                 for (int a = 0; a < 4; a++)
 #pragma unroll
@@ -364,7 +434,7 @@ VIWB_D bool cholesky_packed_rhs(double *L, const int *rp, const int *fst, double
 // back substitution L^T x = y (blocks of 8 from the bottom): every thread that needs it solves the 8x8 triangular block redundantly from
 // broadcast reads (no barrier between the block solve and the update), then the rows above that the block's columns reach (from the
 // block's first stored column on) are updated.  One barrier per block.  Result in y; xo is scratch of n doubles.
-VIWB_D void chol_backsolve_blocked(const double *L, const int *rp, const int *fst, double *y, const double *dinv, double *xo, int n, int tid, int nt,
+VIWB_D void chol_backsolve_blocked(const double *L, const short *rp, const short *fst, double *y, double *xo, int n, int tid, int nt,
                                    SolveClock &sph) {
     (void)sph;
     const int nblk = chol_panels(n);
@@ -386,7 +456,7 @@ VIWB_D void chol_backsolve_blocked(const double *L, const int *rp, const int *fs
                 double v = y[c0 + k];
 #pragma unroll
                 for (int m = 7; m > k; m--) if (m < nb && c0 + k >= fr[m]) v -= rw[m][c0 + k] * x[m];
-                x[k] = v * dinv[c0 + k];
+                x[k] = v * rw[k][c0 + k];          // the inverse pivot
             }
         }
 #pragma unroll
@@ -428,7 +498,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
     WinWork &ww = bd.work[w];
     if (ww.status != ST_RUNNING) return;
     const Opts &op = bd.opt;
-    SolveSmem s; carve(s, smem, nt, bd.env_max);
+    SolveSmem s; carve(s, smem, nt, bd.env_max, bd.nf_max);
     const int nf = m.nf, N = m.nlm, vo = vec_off(bd, w);
     for (int i = tid; i < nf; i += nt) s.fst[i] = m.efirst[i];
     for (int i = tid; i <= nf; i += nt) s.rp[i] = bd.chol_plan[m.plan_off + i];
@@ -442,20 +512,18 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
     const double min_mu = 1e-8, max_mu = 1.0, mu_inc = 10.0;
     SOLVE_PROBE_START();
 
-    // compact <-> fixed / visual index maps
-    for (int b = tid; b < NB; b += nt) if (m.tcol[b] >= 0) for (int k = 0; k < blk_tsize(b); k++) {
-        s.amap[m.tcol[b] + k] = blk_toff(b) + k;
-        s.vmap[m.tcol[b] + k] = blk_voff(b) >= 0 ? blk_voff(b) + k : -1;
-    }
+    // compact -> visual index map
+    for (int b = tid; b < NB; b += nt) if (m.tcol[b] >= 0) for (int k = 0; k < blk_tsize(b); k++) s.vmap[m.tcol[b] + k] = blk_voff(b) >= 0 ? blk_voff(b) + k : -1;
     VIWB_SYNC();
 
     if (mode == 2) { assemble_H(bd, w, s, nf, Hpk, gpk, tid, nt); return; }     // debug hook: normal equations only
     bool assembled = false;
 
     // ================= phase A: decision on the pending candidate ==================================
-    double c_part = 0.0;
-    for (int k = tid; k < N; k += nt) c_part += bd.lm_cost[m.lm_off + k];
-    const double cand_cost = block_sum(c_part, tid, nt, s.red) + ww.small_cost;
+    double c_part[SOLVE_VPT][1] = {};
+    VIWB_VT_LOOP(j, vt) for (int k = vt; k < N; k += SOLVE_VNT) c_part[j][0] += bd.lm_cost[m.lm_off + k];
+    vblock_sum_n<1>(c_part, tid, nt, s.red);
+    const double cand_cost = c_part[0][0] + ww.small_cost;
     bool new_lin = false;
     if (ww.phase == PH_INIT) {
         if (tid == 0) { ww.x_cost = cand_cost; ww.initial_cost = cand_cost; ww.num_iterations = 1; }
@@ -492,11 +560,13 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
     }
     VIWB_SYNC();
     if (new_lin) {   // x_norm over the active blocks
-        double a = 0.0;
-        for (int b = tid; b < NB; b += nt) if (m.tcol[b] >= 0) for (int k = 0; k < blk_size(b); k++) a += x[blk_off(b) + k] * x[blk_off(b) + k];
-        for (int k = tid; k < N; k += nt) a += x[SFIX + k] * x[SFIX + k];
-        a = block_sum(a, tid, nt, s.red);
-        if (tid == 0) ww.x_norm = sqrt(a);
+        double a[SOLVE_VPT][1] = {};
+        VIWB_VT_LOOP(j, vt) {
+            for (int b = vt; b < NB; b += SOLVE_VNT) if (m.tcol[b] >= 0) for (int k = 0; k < blk_size(b); k++) a[j][0] += x[blk_off(b) + k] * x[blk_off(b) + k];
+            for (int k = vt; k < N; k += SOLVE_VNT) a[j][0] += x[SFIX + k] * x[SFIX + k];
+        }
+        vblock_sum_n<1>(a, tid, nt, s.red);
+        if (tid == 0) ww.x_norm = sqrt(a[0][0]);
     }
     if (ww.phase == PH_INIT && op.max_num_iterations <= 0) { VIWB_SYNC(); if (tid == 0) terminate(ww, 1); return; }
     VIWB_SYNC();
@@ -511,20 +581,18 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
             VIWB_SYNC();
             if (tid == 0) ww.reuse = 1;
             if (!assembled) { assemble_H(bd, w, s, nf, Hpk, gpk, tid, nt); assembled = true; }
-            else { load_H(Hpk, s, nf, tid, nt); for (int i = tid; i < nf; i += nt) s.g[i] = gpk[i]; VIWB_SYNC(); }
+            else load_H(Hpk, s, nf, tid, nt);
             SOLVE_MARK(SPH_ASM);
             if (ww.first) {
                 for (int i = tid; i < nf; i += nt) g_scale[i] = op.jacobi_scaling ? 1.0 / (1.0 + sqrt(SKY(s, i, i))) : 1.0;
             }
-            VIWB_SYNC();
-            for (int i = tid; i < nf; i += nt) s.sc[i] = g_scale[i];
             VIWB_SYNC();
             if (new_lin) {
                 // gradient_max_norm = |x - Plus(x, -g)|_inf  (unscaled gradient)
                 double gm = 0.0;
                 for (int b = tid; b < NB; b += nt) if (m.tcol[b] >= 0) {
                     double gneg[9];
-                    for (int k = 0; k < blk_tsize(b); k++) gneg[k] = -s.g[m.tcol[b] + k];
+                    for (int k = 0; k < blk_tsize(b); k++) gneg[k] = -gpk[m.tcol[b] + k];
                     gm = fmax(gm, block_grad_inf(b, m.mask[b], x + blk_off(b), gneg));
                 }
                 for (int k = tid; k < N; k += nt) gm = fmax(gm, fabs(lm_g[k]));
@@ -533,40 +601,45 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 if (gm <= op.gradient_tolerance) { VIWB_SYNC(); if (tid == 0) terminate(ww, 0); return; }
             }
             // D = sqrt(clamp(diag(J_s^T J_s))), scaled gradient, Cauchy direction u_g = c o (sgrad / D)
-            double n2 = 0.0;
-            for (int i = tid; i < nf; i += nt) {
-                double d2 = s.sc[i] * s.sc[i] * SKY(s, i, i);
-                d2 = fmin(fmax(d2, op.min_lm_diagonal), op.max_lm_diagonal);
-                const double D = sqrt(d2); s.D[i] = D; g_D[i] = D;
-                const double sg = s.sc[i] * s.g[i] / D; s.sg[i] = sg; g_sg[i] = sg; n2 += sg * sg;
-                s.ug[i] = s.sc[i] * sg / D;
+            double n2[SOLVE_VPT][1] = {};
+            VIWB_VT_LOOP(j, vt) {
+                for (int i = vt; i < nf; i += SOLVE_VNT) {
+                    const double sc = g_scale[i];
+                    double d2 = sc * sc * SKY(s, i, i);
+                    d2 = fmin(fmax(d2, op.min_lm_diagonal), op.max_lm_diagonal);
+                    const double D = sqrt(d2); g_D[i] = D;
+                    const double sg = sc * gpk[i] / D; g_sg[i] = sg; n2[j][0] += sg * sg;
+                    s.ug[i] = sc * sg / D;
+                }
+                for (int k = vt; k < N; k += SOLVE_VNT) {
+                    const double c = lm_sc[k];
+                    double d2 = c * c * lm_a[k]; d2 = fmin(fmax(d2, op.min_lm_diagonal), op.max_lm_diagonal);
+                    const double D = sqrt(d2); g_D[TFIX + k] = D;
+                    const double sg = c * lm_g[k] / D; g_sg[TFIX + k] = sg; n2[j][0] += sg * sg;
+                }
             }
-            for (int k = tid; k < N; k += nt) {
-                const double c = lm_sc[k];
-                double d2 = c * c * lm_a[k]; d2 = fmin(fmax(d2, op.min_lm_diagonal), op.max_lm_diagonal);
-                const double D = sqrt(d2); g_D[TFIX + k] = D;
-                const double sg = c * lm_g[k] / D; g_sg[TFIX + k] = sg; n2 += sg * sg;
-            }
-            n2 = block_sum(n2, tid, nt, s.red);
+            vblock_sum_n<1>(n2, tid, nt, s.red);
             SOLVE_MARK(SPH_DSC);
             // q_gg = |J u_g|^2, l_g = g . u_g
             symv(s, nf, s.ug, s.Hu, tid, nt);
             to_vis(s, nf, s.ug, s.uvis, tid, nt);
-            double q = 0.0, l = 0.0;
-            for (int i = tid; i < nf; i += nt) { q += s.ug[i] * s.Hu[i]; l += s.g[i] * s.ug[i]; }
-            VIWB_LM_LOOP(k, N) {
-                // the landmark's scalars are fetched (warp-uniform loads) before the dot product so that both latencies overlap
-                const double lsc = lm_sc[k], lsg = g_sg[TFIX + k], lD = g_D[TFIX + k], la = lm_a[k], lg = lm_g[k];
-                const double dw = warp_dot80(W + (size_t)k * VSUB, s.uvis, lane);
-                if (lane == 0) {
-                    wug[k] = dw;
-                    const double ul = lsc * lsg / lD;
-                    q += 2.0 * ul * dw + la * ul * ul;
-                    l += lg * ul;
+            double ql[SOLVE_VPT][2] = {};      // q, l
+            VIWB_VT_LOOP(j, vt) {
+                for (int i = vt; i < nf; i += SOLVE_VNT) { ql[j][0] += s.ug[i] * s.Hu[i]; ql[j][1] += gpk[i] * s.ug[i]; }
+                VIWB_VLM_LOOP(k, vt, N) {
+                    // the landmark's scalars are fetched (warp-uniform loads) before the dot product so that both latencies overlap
+                    const double lsc = lm_sc[k], lsg = g_sg[TFIX + k], lD = g_D[TFIX + k], la = lm_a[k], lg = lm_g[k];
+                    const double dw = warp_dot80(W + (size_t)k * VSUB, s.uvis, lane);
+                    if (lane == 0) {
+                        wug[k] = dw;
+                        const double ul = lsc * lsg / lD;
+                        ql[j][0] += 2.0 * ul * dw + la * ul * ul;
+                        ql[j][1] += lg * ul;
+                    }
                 }
             }
-            { double v2[2] = {q, l}; block_sum_n<2>(v2, tid, nt, s.red); q = v2[0]; l = v2[1]; }
-            if (tid == 0) { ww.sgrad_norm = sqrt(n2); ww.q_gg = q; ww.l_g = l; ww.alpha = n2 / q; }
+            vblock_sum_n<2>(ql, tid, nt, s.red);
+            if (tid == 0) { const double q = ql[0][0], n2s = n2[0][0]; ww.sgrad_norm = sqrt(n2s); ww.q_gg = q; ww.l_g = ql[0][1]; ww.alpha = n2s / q; }
             VIWB_SYNC();
             SOLVE_MARK(SPH_CAUCHY);
             // ---- Gauss-Newton step: (J^T J + mu D^2) y = J^T r through the Schur complement
@@ -581,12 +654,12 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 {
                     for (int i = tid; i < nf; i += nt) {
                         const int vi = s.vmap[i];
-                        double r = s.g[i];
+                        double r = gpk[i];
                         if (vi >= 0) {
                             if (t_ok) r -= tvec[vi];
                             else { double t = 0.0; for (int k = 0; k < N; k++) { const double c = lm_sc[k], sk = c * c * lm_a[k], Dk = g_D[TFIX + k]; t += (c * c / (sk + mu * Dk * Dk)) * W[(size_t)k * VSUB + vi] * lm_g[k]; } r -= t; }
                         }
-                        s.y[i] = s.sc[i] * r;
+                        s.y[i] = g_scale[i] * r;
                     }
                     const int ne = s.rp[nf];
                     for (int e0 = tid; e0 < ne; e0 += SCHUR_U * nt) {
@@ -618,8 +691,8 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                                     hij -= t;
                                 }
                             }
-                            hij *= s.sc[i] * s.sc[j];
-                            if (i == j) hij += mu * s.D[i] * s.D[i];
+                            hij *= g_scale[i] * g_scale[j];
+                            if (i == j) hij += mu * g_D[i] * g_D[i];
                             s.L[e] = hij;
                         }
                     }
@@ -629,16 +702,16 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 SOLVE_COUNT(SPH_FACT);
                 h_dirty = true;
                 if (tid == 0) ww.num_linear++;
-                bool ok = cholesky_packed_rhs(s.L, s.rp, s.fst, s.y, nf, tid, nt, s.chol, s.dinv, s.Pt, bd.chol_plan + m.plan_off, sph);
-                if (ok) chol_backsolve_blocked(s.L, s.rp, s.fst, s.y, s.dinv, s.xo, nf, tid, nt, sph);
+                bool ok = cholesky_packed_rhs(s.L, s.rp, s.fst, s.y, nf, tid, nt, s.chol, s.Pt, s.ldp, bd.chol_plan + m.plan_off, sph);
+                if (ok) chol_backsolve_blocked(s.L, s.rp, s.fst, s.y, s.xo, nf, tid, nt, sph);
                 SOLVE_FLUSH();
                 if (ok) {
                     // back-substitute the inverse depths (scaled): y_k = (c g_k - c w_k . (C y_f)) / h_k
-                    for (int i = tid; i < nf; i += nt) s.u[i] = s.sc[i] * s.y[i];
+                    for (int i = tid; i < nf; i += nt) s.u[i] = g_scale[i] * s.y[i];
                     VIWB_SYNC();
                     to_vis(s, nf, s.u, s.uvis, tid, nt);
                     double bad = 0.0;
-                    for (int i = tid; i < nf; i += nt) { if (!isfinite(s.y[i])) bad = 1.0; g_gn[i] = -s.D[i] * s.y[i]; }
+                    for (int i = tid; i < nf; i += nt) { if (!isfinite(s.y[i])) bad = 1.0; g_gn[i] = -g_D[i] * s.y[i]; }
                     VIWB_LM_LOOP(k, N) {
                         const double c = lm_sc[k], Dk = g_D[TFIX + k], la = lm_a[k], lg = lm_g[k];
                         const double dw = warp_dot80(W + (size_t)k * VSUB, s.uvis, lane);
@@ -650,7 +723,7 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                             g_gn[TFIX + k] = -Dk * yk;
                         }
                     }
-                    bad = block_sum(bad, tid, nt, s.red);
+                    bad = block_sum(bad, tid, nt, s.red);      // a count of non-finite values: exact in any order
                     ok = (bad == 0.0);
                     SOLVE_MARK(SPH_LM2);
                 }
@@ -666,22 +739,25 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 for (int i = tid; i < nf; i += nt) s.u[i] = -s.u[i];
                 VIWB_SYNC();
                 symv(s, nf, s.u, s.Hu, tid, nt);
-                double qnn = 0.0, qgn = 0.0, ln = 0.0, nn = 0.0, gd = 0.0;
-                for (int i = tid; i < nf; i += nt) {
-                    qnn += s.u[i] * s.Hu[i]; qgn += s.ug[i] * s.Hu[i]; ln += s.g[i] * s.u[i];
-                    nn += g_gn[i] * g_gn[i]; gd += s.sg[i] * g_gn[i];
+                double f[SOLVE_VPT][5] = {};      // q_nn, q_gn, l_n, |gn|^2, sgrad . gn
+                VIWB_VT_LOOP(j, vt) {
+                    for (int i = vt; i < nf; i += SOLVE_VNT) {
+                        const double sg = g_sg[i], ug = g_scale[i] * sg / g_D[i];      // the Cauchy direction, as the Cauchy point computed it
+                        f[j][0] += s.u[i] * s.Hu[i]; f[j][1] += ug * s.Hu[i]; f[j][2] += gpk[i] * s.u[i];
+                        f[j][3] += g_gn[i] * g_gn[i]; f[j][4] += sg * g_gn[i];
+                    }
+                    for (int k = vt; k < N; k += SOLVE_VNT) {
+                        const double c = lm_sc[k], Dk = g_D[TFIX + k], ggn = g_gn[TFIX + k], gsg = g_sg[TFIX + k], la = lm_a[k], lg = lm_g[k];
+                        const double dn = -wun[k], dg = wug[k];
+                        const double un = c * ggn / Dk, ug = c * gsg / Dk;
+                        f[j][0] += 2.0 * un * dn + la * un * un;
+                        f[j][1] += ug * dn + un * dg + la * ug * un;
+                        f[j][2] += lg * un;
+                        f[j][3] += ggn * ggn; f[j][4] += gsg * ggn;
+                    }
                 }
-                for (int k = tid; k < N; k += nt) {
-                    const double c = lm_sc[k], Dk = g_D[TFIX + k], ggn = g_gn[TFIX + k], gsg = g_sg[TFIX + k], la = lm_a[k], lg = lm_g[k];
-                    const double dn = -wun[k], dg = wug[k];
-                    const double un = c * ggn / Dk, ug = c * gsg / Dk;
-                    qnn += 2.0 * un * dn + la * un * un;
-                    qgn += ug * dn + un * dg + la * ug * un;
-                    ln += lg * un;
-                    nn += ggn * ggn; gd += gsg * ggn;
-                }
-                { double v5[5] = {qnn, qgn, ln, nn, gd}; block_sum_n<5>(v5, tid, nt, s.red); qnn = v5[0]; qgn = v5[1]; ln = v5[2]; nn = v5[3]; gd = v5[4]; }
-                if (tid == 0) { ww.q_nn = qnn; ww.q_gn = qgn; ww.l_n = ln; ww.gn_norm = sqrt(nn); ww.sgrad_dot_gn = gd; }
+                vblock_sum_n<5>(f, tid, nt, s.red);
+                if (tid == 0) { ww.q_nn = f[0][0]; ww.q_gn = f[0][1]; ww.l_n = f[0][2]; ww.gn_norm = sqrt(f[0][3]); ww.sgrad_dot_gn = f[0][4]; }
             }
             VIWB_SYNC();
             SOLVE_MARK(SPH_FORMS);
@@ -727,8 +803,9 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
             continue;
         }
         // ---- candidate: x (+) (step o scale)
-        double sn = 0.0;
-        for (int b = tid; b < NB; b += nt) {
+        double sn[SOLVE_VPT][1] = {};
+        VIWB_VT_LOOP(j, vt) {
+        for (int b = vt; b < NB; b += SOLVE_VNT) {
             const int o = blk_off(b), gs = blk_size(b);
             if (m.tcol[b] >= 0) {
                 double d[9], out[9];
@@ -736,16 +813,17 @@ VIWB_D void solve_block(const BatchDev &bd, int bx, int by, int tid, int nt, dou
                 if (gs == 7) pose_plus(x + o, d, m.mask[b], out);
                 else if (gs == 4) quat_plus(x + o, d, m.mask[b], out);
                 else for (int k = 0; k < gs; k++) out[k] = x[o + k] + d[k];
-                for (int k = 0; k < gs; k++) { xc[o + k] = out[k]; const double e = x[o + k] - out[k]; sn += e * e; }
+                for (int k = 0; k < gs; k++) { xc[o + k] = out[k]; const double e = x[o + k] - out[k]; sn[j][0] += e * e; }
             } else for (int k = 0; k < gs; k++) xc[o + k] = x[o + k];
         }
-        for (int k = tid; k < N; k += nt) {
+        for (int k = vt; k < N; k += SOLVE_VNT) {
             const double d = (ca * g_sg[TFIX + k] + cb * g_gn[TFIX + k]) / g_D[TFIX + k] * lm_sc[k];
-            xc[SFIX + k] = x[SFIX + k] + d; sn += d * d;
+            xc[SFIX + k] = x[SFIX + k] + d; sn[j][0] += d * d;
         }
-        sn = block_sum(sn, tid, nt, s.red);
+        }
+        vblock_sum_n<1>(sn, tid, nt, s.red);
         if (tid == 0) {
-            ww.num_invalid = 0; ww.step_norm = sqrt(sn); ww.model_cost_change = mcc; ww.dogleg_step_norm = dsn;
+            ww.num_invalid = 0; ww.step_norm = sqrt(sn[0][0]); ww.model_cost_change = mcc; ww.dogleg_step_norm = dsn;
             ww.phase = PH_CAND;
             ww.mu_lin = fmax(min_mu, 2.0 * ww.mu / mu_inc);      // the candidate's linearisation is solved with the post-accept mu
         }

@@ -105,7 +105,7 @@ struct Opts {
 
 struct BatchDev {       // passed by value to every kernel
     int B, nvis_total, nlm_total, nimu_total, nwheel_total, nplane_total, nprior, nitems_solve, nitems_marg;
-    int env_max;            // largest esize over the batch (sizes the solve kernel's shared memory)
+    int env_max, nf_max;    // largest esize and nf over the batch (size the solve kernel's shared memory)
     int marg_nmax;          // largest prior dimension any window of the batch produces (sizes the eigen-solver's shared memory)
     int n_unfused;          // windows whose solver linearisation runs lin_vis + lm_reduce + asm_items (the others: lin_vis_lm(_wide), WinMeta.fused)
     int n_fused_wide, n_fused_compact, n_munfused, n_mfused;      // fused solver windows by record width; marginalising windows by path

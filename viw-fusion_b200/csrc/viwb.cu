@@ -99,10 +99,12 @@ DEF_KERNEL(lm_reduce, 128)
 #endif
 DEF_KERNEL2(lin_small, 128, LSM_MINB)
 DEF_KERNEL(asm_items, 128)
-#ifndef SOLVE_NT
-#define SOLVE_NT 384
-#endif
-DEF_KERNEL2(solve, SOLVE_NT, 2)
+// SOLVE_NT (kernels_solve.cuh): 256 threads and a C2 window's shared memory fit three windows per SM.  solve_wide runs the same block function
+// with 384 threads, two per SM, for batches whose widest window leaves no room for a third block (solve_threads); -DSOLVE_NT=384 builds both at 384.
+DEF_KERNEL2(solve, SOLVE_NT, SOLVE_NT <= 256 ? 3 : 2)
+enum { SOLVE_WIDE_NT = 384 };
+VIWB_D void solve_wide_block(const BatchDev &bd, int bx, int by, int tid, int nt, double *smem, int mode) { solve_block(bd, bx, by, tid, nt, smem, mode); }
+DEF_KERNEL2(solve_wide, SOLVE_WIDE_NT, 2)
 #ifndef LVL_MINB
 #define LVL_MINB 4
 #endif
@@ -184,7 +186,8 @@ static int launch_status(viwb_context *ctx) {
 static int ensure_attrs(viwb_context *ctx) {
 #ifndef VIWB_HOST_EMU
     if (!ctx->attrs_set) {
-        CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_NT, TFIX * (TFIX + 1) / 2) * 8)));
+        CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_NT, TFIX * (TFIX + 1) / 2, TFIX) * 8)));
+        CK(cudaFuncSetAttribute(solve_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(solve_smem_doubles(SOLVE_WIDE_NT, TFIX * (TFIX + 1) / 2, TFIX) * 8)));
         CK(cudaFuncSetAttribute(lin_vis_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_smem_doubles(128) * 8)));
         CK(cudaFuncSetAttribute(lin_vis_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_run_smem_doubles() * 8)));
         CK(cudaFuncSetAttribute(lin_vis_lm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(lin_vis_lm_smem_doubles(true) * 8)));
@@ -778,7 +781,8 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     bd.pitems_max = 1; for (int w = 0; w < B; w++) bd.pitems_max = std::max(bd.pitems_max, std::max(b->meta[w].npitems, b->meta[w].nmpitems));
     bd.pout_stride = bd.n_fused_wide ? (int)XL<true>::OUT : (int)XL<false>::OUT;
     bd.marg_nmax = b->prior_nmax;
-    bd.env_max = 1; for (int w = 0; w < B; w++) bd.env_max = std::max(bd.env_max, b->meta[w].esize);
+    bd.env_max = 1; bd.nf_max = 1;
+    for (int w = 0; w < B; w++) { bd.env_max = std::max(bd.env_max, b->meta[w].esize); bd.nf_max = std::max(bd.nf_max, b->meta[w].nf); }
     b->total_state = nstate;
     // ---- the slab: every array once -- its device field, its element count, and for an input its view in the staging slab (HostArrays).
     // Inputs come first and are uploaded as one block; a work array is never empty.
@@ -856,6 +860,20 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
 
 enum { RUN_SOLVE = 1, RUN_REANCHOR = 2, RUN_MARG = 4, RUN_LIN_ONLY = 8 };
 
+// Threads per block of the batch's solve launch: SOLVE_NT, unless the widest window's shared memory leaves that kernel fewer resident warps per SM
+// than the 384-thread one (both hold two such windows per SM, as for C4 windows): then SOLVE_WIDE_NT.  The emulation always runs solve_block.
+static int solve_threads(const BatchDev &bd) {
+#ifdef VIWB_HOST_EMU
+    (void)bd;
+    return SOLVE_NT;
+#else
+    int a = 0, b = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, solve_kernel, SOLVE_NT, solve_smem_doubles(SOLVE_NT, bd.env_max, bd.nf_max) * 8) ||
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, solve_wide_kernel, SOLVE_WIDE_NT, solve_smem_doubles(SOLVE_WIDE_NT, bd.env_max, bd.nf_max) * 8))
+        return SOLVE_NT;
+    return a * SOLVE_NT >= b * SOLVE_WIDE_NT ? SOLVE_NT : SOLVE_WIDE_NT;
+#endif
+}
 static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
     bind_device(ctx);
     BatchDev &bd = b->bd;
@@ -868,7 +886,7 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
     CK(dev_d2d(bd.work, b->work_init_dev, sizeof(WinWork) * B, st));
     const int nt_vis = NT(128), nt_lm = NT(128), nt_small = NT(128), nt_asm = NT(128), nt_solve = NT(SOLVE_NT), nt_marg = NT(256);
     const int g_vis = (bd.nvis_total + nt_vis - 1) / nt_vis, g_lm = (bd.nlm_total * LM_ROLES + nt_lm - 1) / nt_lm;
-    const size_t sm_small = lin_small_smem_doubles(nt_small) * 8, sm_solve = solve_smem_doubles(nt_solve, bd.env_max) * 8, sm_marg = marg_prep_smem_doubles(nt_marg, bd.marg_nmax) * 8, sm_eig = marg_eig_smem_doubles(nt_marg, bd.marg_nmax) * 8;
+    const size_t sm_small = lin_small_smem_doubles(nt_small) * 8, sm_solve = solve_smem_doubles(nt_solve, bd.env_max, bd.nf_max) * 8, sm_marg = marg_prep_smem_doubles(nt_marg, bd.marg_nmax) * 8, sm_eig = marg_eig_smem_doubles(nt_marg, bd.marg_nmax) * 8;
     // cost_only: the round after the last allowed iteration only decides accept / reject of the pending candidate (every window
     // still running is at max_num_iterations there, trust_region_minimizer.cc checks the iteration limit before the gradient),
     // so the partial sums and the Schur product of that linearisation would never be read
@@ -899,7 +917,14 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
         LAUNCH(ctx, setup, bd, (ns + nt_s - 1) / nt_s, 1, nt_s, 0, 0);
         LAUNCH(ctx, prior_setup, bd, bd.nprior, 1, NT(256), 0, 0);
     }
-    if (what & RUN_LIN_ONLY) { lin(MODE_SOLVE, false); LAUNCH(ctx, solve, bd, B, 1, nt_solve, sm_solve, 2); }
+    // the solve kernel at the block size that keeps more of its warps resident (solve_threads); both compute the same bits
+    const int solve_nt = solve_threads(bd);
+    const size_t sm_solve_at = solve_smem_doubles(solve_nt, bd.env_max, bd.nf_max) * 8;
+    auto launch_solve = [&](int mode) {
+        if (solve_nt == SOLVE_NT) LAUNCH(ctx, solve, bd, B, 1, nt_solve, sm_solve, mode);
+        else KERNEL(ctx, "solve", B, 1, solve_nt, sm_solve_at, solve_wide_kernel, (bd, mode), emu_launch(solve_block, bd, B, 1, sm_solve_at, mode));
+    };
+    if (what & RUN_LIN_ONLY) { lin(MODE_SOLVE, false); launch_solve(2); }
     if (what & RUN_SOLVE) {
         // SOLVER_TIME (estimator.cpp:1650-1653): Ceres tests the wall clock after every iteration; here the host
         // waits for each round only when a limit is set, and the round after the limit just decides the pending
@@ -912,7 +937,7 @@ static int batch_execute(viwb_context *ctx, viwb_batch *b, int what) {
                 last = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_start).count() >= b->max_time;
             }
             lin(MODE_SOLVE, last || (round == b->max_iter && round > 0));
-            LAUNCH(ctx, solve, bd, B, 1, nt_solve, sm_solve, last ? 3 : 0);
+            launch_solve(last ? 3 : 0);
         }
     }
     if (what & RUN_REANCHOR) LAUNCH(ctx, reanchor, bd, B, 1, NT(32), 0, 0);
@@ -1127,6 +1152,22 @@ extern "C" int viwb_batch_outliers(viwb_context *ctx, viwb_batch *b, double foca
     return VIWB_OK;
 }
 extern "C" double viwb_batch_algorithmic_bytes(const viwb_batch *b) { return b ? b->algorithmic_bytes : 0.0; }
+extern "C" int viwb_batch_solve_launch(viwb_context *ctx, const viwb_batch *b, int *threads, int *smem_bytes, int *blocks_per_sm) {
+    if (!ctx || !b) return fail(ctx, VIWB_ERR_INVALID, "viwb_batch_solve_launch: null argument");
+    bind_device(ctx);
+    int rc = ensure_attrs(ctx); if (rc) return rc;
+    const int nt = solve_threads(b->bd), smem = (int)(solve_smem_doubles(nt, b->bd.env_max, b->bd.nf_max) * 8);
+    if (threads) *threads = nt;
+    if (smem_bytes) *smem_bytes = smem;
+    if (blocks_per_sm) {
+#ifdef VIWB_HOST_EMU
+        return fail(ctx, VIWB_ERR_INVALID, "viwb_batch_solve_launch: no device in the emulation");
+#else
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(blocks_per_sm, nt == SOLVE_NT ? (const void *)solve_kernel : (const void *)solve_wide_kernel, nt, (size_t)smem));
+#endif
+    }
+    return VIWB_OK;
+}
 extern "C" void viwb_batch_destroy(viwb_context *ctx, viwb_batch *b) { batch_free(ctx, b); }
 
 static int run_once(viwb_context *ctx, int B, const viwb_problem *problems, double *const *states, const viwb_options *opt,

@@ -17,7 +17,7 @@ DEFAULT_LIB = os.path.normpath(os.path.join(_HERE, "..", "..", "csrc", "libviwb.
 EXPORTS = ["viwb_create", "viwb_destroy", "viwb_last_error", "viwb_set_stream", "viwb_launch_count", "viwb_h2d_bytes", "viwb_set_profiling", "viwb_profile_count", "viwb_profile_get", "viwb_default_options",
            "viwb_default_globals", "viwb_factor_evaluate", "viwb_prior_evaluate", "viwb_window_solve", "viwb_gauge_reanchor",
            "viwb_marginalize", "viwb_optimization", "viwb_optimization_batch", "viwb_batch_create", "viwb_batch_reset_states",
-           "viwb_batch_run", "viwb_batch_download", "viwb_batch_algorithmic_bytes", "viwb_batch_destroy",
+           "viwb_batch_run", "viwb_batch_download", "viwb_batch_algorithmic_bytes", "viwb_batch_solve_launch", "viwb_batch_destroy",
            "viwb_debug_normal_equations", "viwb_lk_track", "viwb_track_checked", "viwb_lk_batch_create", "viwb_lk_batch_destroy",
            "viwb_lk_batch_upload", "viwb_lk_batch_run", "viwb_lk_batch_download", "viwb_lk_batch_algorithmic_bytes", "viwb_host_register",
            "viwb_host_unregister", "viwb_imu_preintegrate", "viwb_wheel_preintegrate", "viwb_outlier_rejection", "viwb_batch_outliers", "viwb_triangulate", "viwb_shift_depth", "viwb_predict_pts", "viwb_undistort_velocity", "viwb_undistort_velocity_camera",
@@ -801,6 +801,13 @@ class Batch:
 
     def algorithmic_bytes(self):
         return float(self.ctx.lib.viwb_batch_algorithmic_bytes(self.h))
+
+    def solve_launch(self, occupancy=True):
+        """(threads per block, dynamic shared-memory bytes, blocks per SM or None) of this batch's solve kernel (viwb_batch_solve_launch)."""
+        nt, sm, bps = C.c_int(), C.c_int(), C.c_int()
+        self.ctx._ck(self.ctx.lib.viwb_batch_solve_launch(self.ctx.h, self.h, C.byref(nt), C.byref(sm), C.byref(bps) if occupancy else None),
+                     "viwb_batch_solve_launch")
+        return nt.value, sm.value, (bps.value if occupancy else None)
 
     def download(self, want_priors=True):
         sts = [np.zeros(p.state_size) for p in self.problems]
