@@ -590,6 +590,30 @@ int viwb_features_remove_failures(viwb_features *fs);
  * [..][11], is_stereo [..][11].  Entries past n[s] or num_obs are undefined.  Any pointer may be NULL.  Synchronises. */
 int viwb_features_download(viwb_features *fs, int32_t *n, int32_t *ids, int32_t *start_frame, int32_t *num_obs, double *depth, int32_t *solve_flag,
                            float *obs, double *cur_td, uint8_t *is_stereo);
+/* optimization()'s visual loop + getDepthVector + viwb_batch_create in one call: one window per stream, in stream order, its visual factors
+ * and landmark inverse depths taken from the lists in HBM.  problems[s] carries everything else (frame_count, block flags / masks, IMU /
+ * wheel / plane tables, prior, globals) with num_vis == 0, num_landmarks == 0 and NULL visual tables; states [streams][VIWB_STATE_FIXED].
+ * margin_flags as in viwb_batch_create (NULL: no marginalisation).  num_landmarks [streams] (may be NULL): each window's landmark count.
+ * The result is an ordinary viwb_batch (run / reset_states / download / outliers / destroy unchanged) and counts as an export for
+ * set_depth / remove_outliers.  Only a digest of a few bytes per landmark crosses the bus, and the batch's upload leaves out the observations
+ * and the landmark states, so the windows are bit for bit those of viwb_features_window + viwb_batch_create.  VIWB_ERR_INVALID with no batch
+ * made: an add error still unread, a stream with more than VIWB_MAX_LANDMARKS landmarks, a problem with visual rows or landmarks, a list
+ * observation beyond the problem's frame_count, or any refusal of viwb_batch_create.  Synchronises. */
+int viwb_features_batch_create(viwb_features *fs, const viwb_problem *problems, const double *states, const viwb_options *options,
+                               const int32_t *margin_flags, int32_t *num_landmarks, viwb_batch **out);
+/* The feedback calls below take a batch of viwb_features_batch_create on these lists (VIWB_ERR_INVALID for a batch of other lists or of
+ * viwb_batch_create) and read it in HBM. */
+/* setDepth from the batch's current landmark states (after viwb_batch_run: the solution), device to device: the function of
+ * viwb_features_set_depth fed them.  VIWB_ERR_INVALID if a list changed since the batch's create. */
+int viwb_features_set_depth_batch(viwb_features *fs, const viwb_batch *b);
+/* outliersRejection on the batch (the verdicts viwb_batch_outliers gives) + removeOutlier, without the verdicts crossing the bus; outputs as
+ * viwb_features_remove_outliers.  VIWB_ERR_INVALID if a list changed since the batch's create.  Synchronises. */
+int viwb_features_remove_outliers_batch(viwb_features *fs, viwb_batch *b, double focal_length, double threshold_px,
+                                        int32_t *n_removed, int32_t *removed_ids);
+/* predictPtsInNextFrame with each stream's fixed state read from the batch; outputs as viwb_features_predict.  Only the fixed states are
+ * read, so it follows remove_outliers_batch as predictPtsInNextFrame follows removeOutlier in processImage.  Synchronises. */
+int viwb_features_predict_batch(viwb_features *fs, const viwb_batch *b, const int32_t *frame_count, int32_t *n_pred, int32_t *pred_ids,
+                                double *pred_pts_cam, uint8_t *has_prediction);
 
 /* Page-lock / unlock caller-owned host memory (camera frame buffers) for asynchronous full-rate uploads. */
 int viwb_host_register(viwb_context *ctx, void *ptr, size_t bytes);

@@ -11,6 +11,7 @@
 // slot's cur_td and its is_stereo flag.  Erasing features is a stable compaction from one buffer into the other (the host flips them).
 #pragma once
 #include "kernels_feat.cuh"
+#include "layout.cuh"
 
 namespace viwb {
 
@@ -34,10 +35,14 @@ struct FmRun {
     FmRows rows; const int *fc; const double *td;         // add: rows, frame_count [F], td [F]
     const double *state;                    // [F][207] triangulate / predict
     const int *off; const double *xin; const unsigned char *verdict;      // set_depth / outliers: landmark k of stream s at off[s] + k
+    const int *verdict_i;                   // outliers from a batch: its int verdicts (lm_outlier) in place of `verdict`
+    const int *st_off;                      // predict from a batch: stream s's fixed state at state + st_off[s] (NULL: s * 207)
     const unsigned char *shift; const double *mats;       // slide: [F] flags, [F][24] = marg_R 9, marg_P 3, new_R 9, new_P 3
     int *o_cnt, *o_ids; double *o_pts;      // [F], [F][M], [F][M][3]: removed ids / predictions
     const int *w_off;                       // window: [F][2] packed row / landmark offsets
     int *w_type, *w_lm, *w_fi, *w_fj, *w_id; double *w_obs, *w_inv;
+    unsigned *w_dig;                        // window digest: one word per landmark at w_off[s] (fm_digest_word)
+    const WinMeta *b_meta; const int *b_oi; double *b_obs_i, *b_obs_j, *b_x; const double *b_xfix;      // batch fill: window s of a batch slab
 };
 
 VIWB_HD int fm_imin(int a, int b) { return a < b ? a : b; }
@@ -242,6 +247,31 @@ VIWB_D int fm_rows_of(const FmRun &r, size_t f) {
     return c;
 }
 
+// The visual factors of one landmark in the order of estimator.cpp:1585-1638: per observation slot j, the left camera (2F1C, from slot 1 on), then on
+// a stereo slot the right one (2F2C, or 1F2C on slot 0).  ster: bit j = slot j is stereo (and the configuration is).
+// visit(slot, camera, VIWB_F_PROJ_2F1C / 2F2C / 1F2C, imu_i, imu_j).  The export, the batch fill and the host lowering of a digest all enumerate here.
+#ifdef __CUDACC__
+#pragma nv_exec_check_disable      // the host lowering's visitor is a host lambda; the kernels' are device lambdas
+#endif
+template <typename V>
+VIWB_HD void fm_factors(int start, int nobs, unsigned ster, V visit) {
+    for (int j = 0; j < nobs; j++)
+        for (int cam = 0; cam < 2; cam++) {
+            if (cam == 0 ? j == 0 : !((ster >> j) & 1u)) continue;
+            visit(j, cam, cam == 0 ? 0 : (j != 0 ? 1 : 2), start, start + j);
+        }
+}
+VIWB_D unsigned fm_ster_mask(const FmRun &r, size_t f) {
+    unsigned m = 0;
+    if (r.stereo) for (int j = 0; j < r.src.nobs[f]; j++) m |= (unsigned)r.src.ster[f * FM_SLOTS + j] << j;
+    return m;
+}
+// digest word of a landmark: start frame (4 bits), observation count (4 bits), stereo mask (FM_SLOTS bits)
+VIWB_HD unsigned fm_digest_word(int start, int nobs, unsigned ster) { return (unsigned)start | (unsigned)nobs << 4 | ster << 8; }
+VIWB_HD int fm_digest_start(unsigned d) { return (int)(d & 15u); }
+VIWB_HD int fm_digest_nobs(unsigned d) { return (int)((d >> 4) & 15u); }
+VIWB_HD unsigned fm_digest_ster(unsigned d) { return d >> 8; }
+
 // ---- window, launch 1 of 2: landmarks and visual rows per stream
 VIWB_D void fm_window_count(const FmRun &r, int s, int tid, int nt, int *sc) {
     const size_t base = (size_t)s * r.M;
@@ -259,26 +289,58 @@ VIWB_D void fm_window_write(const FmRun &r, int s, int tid, int nt, int *sc) {
     fm_number(r, s, tid, nt, sc);
     fm_scan(r.n[s], tid, nt, sc, [&](int k) { return fm_rows_of(r, base + k); }, [&](int k, int o) {
         const size_t f = base + k;
-        const int l = lm[k], imu_i = L.start[f];
+        const int l = lm[k];
         r.w_inv[lm0 + l] = trk_div(1.0, L.depth[f]); r.w_id[lm0 + l] = L.id[f];
         const float *o0 = L.obs + f * FM_SLOTS * FM_OBS;
         int q = row0 + o;
-        for (int j = 0; j < L.nobs[f]; j++) {
-            const int imu_j = imu_i + j;
-            const float *oj = o0 + (size_t)j * FM_OBS;
-            for (int cam = 0; cam < 2; cam++) {
-                if (cam == 0 ? j == 0 : !(r.stereo && L.ster[f * FM_SLOTS + j])) continue;
-                const float *pj = oj + 6 * cam;
-                double *ob = r.w_obs + (size_t)q * 12;
-                ob[0] = (double)o0[0]; ob[1] = (double)o0[1]; ob[2] = 1.0;
-                ob[3] = (double)pj[0]; ob[4] = (double)pj[1]; ob[5] = 1.0;
-                ob[6] = (double)o0[4]; ob[7] = (double)o0[5]; ob[8] = (double)pj[4]; ob[9] = (double)pj[5];
-                ob[10] = L.td[f * FM_SLOTS]; ob[11] = L.td[f * FM_SLOTS + j];
-                r.w_type[q] = cam == 0 ? 0 : (j != 0 ? 1 : 2);                    // VIWB_F_PROJ_2F1C / 2F2C / 1F2C
-                r.w_lm[q] = l; r.w_fi[q] = imu_i; r.w_fj[q] = imu_j;
-                q++;
-            }
-        }
+        fm_factors(L.start[f], L.nobs[f], fm_ster_mask(r, f), [&](int j, int cam, int type, int imu_i, int imu_j) {
+            const float *pj = o0 + (size_t)j * FM_OBS + 6 * cam;
+            double *ob = r.w_obs + (size_t)q * 12;
+            ob[0] = (double)o0[0]; ob[1] = (double)o0[1]; ob[2] = 1.0;
+            ob[3] = (double)pj[0]; ob[4] = (double)pj[1]; ob[5] = 1.0;
+            ob[6] = (double)o0[4]; ob[7] = (double)o0[5]; ob[8] = (double)pj[4]; ob[9] = (double)pj[5];
+            ob[10] = L.td[f * FM_SLOTS]; ob[11] = L.td[f * FM_SLOTS + j];
+            r.w_type[q] = type; r.w_lm[q] = l; r.w_fi[q] = imu_i; r.w_fj[q] = imu_j;
+            q++;
+        });
+    });
+}
+
+// ---- window digest (viwb_features_batch_create, after fm_window_count): one word per landmark, in the export's numbering, at w_off[s]
+VIWB_D void fm_window_digest(const FmRun &r, int s, int tid, int nt, int *sc) {
+    const size_t base = (size_t)s * r.M;
+    const FmList &L = r.src;
+    const int l0 = r.w_off[s];
+    fm_scan(r.n[s], tid, nt, sc, [&](int k) { return L.nobs[base + k] >= 4 ? 1 : 0; }, [&](int k, int l) {
+        const size_t f = base + k;
+        r.w_dig[l0 + l] = fm_digest_word(L.start[f], L.nobs[f], fm_ster_mask(r, f));
+    });
+}
+
+// ---- batch fill: the observations and inverse depths of window s of a batch built from the digest, straight into its slab in the wire format
+// (kernels_lin.cuh vis_expand reads them next): the host side once per landmark from its first observation, at the index the lowering gave the
+// landmark's first factor, the observer side per factor, x_init's landmark part as fm_window_write's 1 / estimated_depth beside the uploaded
+// fixed state
+VIWB_D void fm_batch_fill(const FmRun &r, int s, int tid, int nt, int *sc) {
+    const size_t base = (size_t)s * r.M;
+    const FmList &L = r.src;
+    const WinMeta &m = r.b_meta[s];
+    const int *lm = r.iscr + base;
+    for (int k = tid; k < SFIX; k += nt) r.b_x[m.state_off + k] = r.b_xfix[(size_t)s * SFIX + k];
+    fm_number(r, s, tid, nt, sc);
+    fm_scan(r.n[s], tid, nt, sc, [&](int k) { return fm_rows_of(r, base + k); }, [&](int k, int o) {
+        const size_t f = base + k;
+        r.b_x[m.state_off + SFIX + lm[k]] = trk_div(1.0, L.depth[f]);
+        const float *o0 = L.obs + f * FM_SLOTS * FM_OBS;
+        int q = m.vis_off + o;
+        double *hi = r.b_obs_i + (size_t)r.b_oi[q] * 6;
+        hi[0] = (double)o0[0]; hi[1] = (double)o0[1]; hi[2] = 1.0; hi[3] = (double)o0[4]; hi[4] = (double)o0[5]; hi[5] = L.td[f * FM_SLOTS];
+        fm_factors(L.start[f], L.nobs[f], fm_ster_mask(r, f), [&](int j, int cam, int, int, int) {
+            const float *pj = o0 + (size_t)j * FM_OBS + 6 * cam;
+            double *hj = r.b_obs_j + (size_t)q * 6;
+            hj[0] = (double)pj[0]; hj[1] = (double)pj[1]; hj[2] = 1.0; hj[3] = (double)pj[4]; hj[4] = (double)pj[5]; hj[5] = L.td[f * FM_SLOTS + j];
+            q++;
+        });
     });
 }
 
@@ -305,7 +367,7 @@ VIWB_D void fm_predict(const FmRun &r, int s, int tid, int nt, int *sc) {
         const float *o = L.obs + (base + k) * FM_SLOTS * FM_OBS;
         double p0[3] = {(double)o[0], (double)o[1], 1.0};
         unsigned char v;
-        PredictArgs a; a.n = 1; a.frame_count = r.fc[s]; a.state = r.state + (size_t)s * 207; a.start_frame = L.start + base + k; a.num_obs = L.nobs + base + k;
+        PredictArgs a; a.n = 1; a.frame_count = r.fc[s]; a.state = r.state + (r.st_off ? (size_t)r.st_off[s] : (size_t)s * 207); a.start_frame = L.start + base + k; a.num_obs = L.nobs + base + k;
         a.pt0 = p0; a.depth = L.depth + base + k; a.pts_cam = pts + 3 * k; a.valid = &v;
         predict_pts_item(a, 0);
         ok[k] = v;
@@ -338,7 +400,7 @@ VIWB_D void fm_compact(const FmRun &r, int s, int tid, int nt, int *sc) {
         double dep = A.depth[f];
         if (r.mode == FM_COMPACT_OUTLIERS) {
             const int l = plan[k];
-            p = (l >= 0 && r.verdict[r.off[s] + l]) ? 0 : 1;
+            p = (l >= 0 && (r.verdict ? r.verdict[r.off[s] + l] != 0 : r.verdict_i[r.off[s] + l] != 0)) ? 0 : 1;
         } else if (r.mode == FM_COMPACT_FAILURES) {
             p = A.flag[f] == 2 ? 0 : 1;
         } else if (fc == VIWB_WINDOW_SIZE) {
@@ -394,6 +456,8 @@ __global__ void __launch_bounds__(FM_NT) fm_add_apply_kernel(FmRun r) { __shared
 __global__ void __launch_bounds__(FM_NT) fm_triangulate_kernel(FmRun r) { fm_triangulate(r, blockIdx.x, threadIdx.x, blockDim.x); }
 __global__ void __launch_bounds__(FM_NT) fm_window_count_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_window_count(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }
 __global__ void __launch_bounds__(FM_NT) fm_window_write_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_window_write(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }
+__global__ void __launch_bounds__(FM_NT) fm_window_digest_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_window_digest(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }
+__global__ void __launch_bounds__(FM_NT) fm_batch_fill_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_batch_fill(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }
 __global__ void __launch_bounds__(FM_NT) fm_set_depth_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_set_depth(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }
 __global__ void __launch_bounds__(FM_NT) fm_predict_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_predict(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }
 __global__ void __launch_bounds__(FM_NT) fm_compact_kernel(FmRun r) { __shared__ int sc[FM_NT + 2]; fm_compact(r, blockIdx.x, threadIdx.x, blockDim.x, sc); }

@@ -262,6 +262,10 @@ struct viwb_batch {
     bool any_marg;
     int max_iter;
     double max_time;       // max_solver_time_in_seconds (0 = off): checked on the host between rounds, like Ceres' wall-clock test
+    // viwb_features_batch_create: the lists it was built from and their generation then; x_fix [B][SFIX] the uploaded fixed states (the fill copies
+    // them into x_init beside the landmarks), fm_off [2][B] each window's state_off and lm_off for the feedback kernels.  NULL / unused otherwise.
+    const viwb_features *fs; long long fs_gen;
+    double *x_fix; int *fm_off;
 };
 
 static void opts_from(const viwb_options *o, Opts &d) {
@@ -307,6 +311,7 @@ enum SolvePath { SOLVE_UNFUSED, SOLVE_COMPACT, SOLVE_WIDE };      // lin_vis + l
 enum MargPath { MARG_NONE, MARG_UNFUSED, MARG_WIDE };             // none: no visual factor is marginalised (window not full, no flag, or MARGIN_SECOND_NEW)
 struct WinLow {
     int err; bool grouped, has_prior;
+    bool dev_obs;                                     // the observations and inverse depths are filled on the device (fm_batch_fill), vis_obs is NULL
     int prior_n_out;
     bool obs_per_factor; int nobs_i, obsi_off;       // entries of the host-side observation table (wire format): one per run of factors with an identical (pts_i, velocity_i, td_i)
     int solve, marg;                                  // SolvePath, MargPath
@@ -343,11 +348,12 @@ template <typename F> static void host_runs(int nvis, const int *vl, const int *
     }
 }
 
-static void lower_count(const viwb_problem &p, int mf, bool allow_fused, WinMeta &m, WinLow &lo, int &out_mode) {
+static void lower_count(const viwb_problem &p, int mf, bool allow_fused, bool dev_obs, WinMeta &m, WinLow &lo, int &out_mode) {
     memset(&m, 0, sizeof m); memset(&lo, 0, sizeof lo);
+    lo.dev_obs = dev_obs;
     if (p.frame_count < 0 || p.frame_count > VIWB_WINDOW_SIZE || p.num_landmarks < 0 || p.num_landmarks > VIWB_MAX_LANDMARKS) { lo.err = 1; return; }
     if (p.num_vis < 0 || p.num_imu < 0 || p.num_wheel < 0 || p.num_plane < 0) { lo.err = 5; return; }            // counts are added up as size_t below
-    if ((p.num_vis && (!p.vis_type || !p.vis_landmark || !p.vis_frame_i || !p.vis_frame_j || !p.vis_obs)) || (p.num_imu && (!p.imu_frame_i || !p.imu_frame_j || !p.imu_data)) ||
+    if ((p.num_vis && (!p.vis_type || !p.vis_landmark || !p.vis_frame_i || !p.vis_frame_j || (!p.vis_obs && !dev_obs))) || (p.num_imu && (!p.imu_frame_i || !p.imu_frame_j || !p.imu_data)) ||
         (p.num_wheel && (!p.wheel_frame_i || !p.wheel_frame_j || !p.wheel_data)) || (p.num_plane && !p.plane_frame)) { lo.err = 5; return; }
     m.nlm = p.num_landmarks; m.frame_count = p.frame_count; m.nvis = p.num_vis; m.nimu = p.num_imu; m.nwheel = p.num_wheel; m.nplane = p.num_plane;
     for (int k = 0; k < 3; k++) m.G[k] = p.globals.G[k];
@@ -507,10 +513,10 @@ static void lower_count(const viwb_problem &p, int mf, bool allow_fused, WinMeta
 
 // ---- phase 3: fill this window's slices of the (pinned) staging arrays; every offset is final
 struct HostArrays {      // the input arrays' views in the staging slab (batch_build's slab table sets them)
-    WinMeta *meta; PriorDev *prior; int *vis_code, *vis_lm, *vis_oi; double *obs_i, *obs_j; int *lm_win, *lm_fptr;
+    WinMeta *meta; PriorDev *prior; int *vis_code, *vis_lm, *vis_oi; double *obs_i, *obs_j; int *lm_win, *lm_fptr; double *x_fix; int *fm_off;
     AsmItem *items; int *asm_list; int *imu_fi, *imu_fj, *imu_win, *wheel_fi, *wheel_fj, *wheel_win, *plane_f, *plane_win;
     double *imu_data, *wheel_data, *prior_J, *prior_r, *prior_x0, *x_init; WinWork *work;
-    int nitems_solve_total;
+    int nitems_solve_total, meta_count;
     int *vis_pos; LmbDesc *lmb_desc; AsmItem *pitems; int *mvis_pos; AsmItem *mpitems;
     RunDesc *run_desc; RunTile *run_tile; int *run_f, *run_lm;
     unsigned char *obs_viol;        // [B] host only: set by lower_fill when a grouped table does not share one host-side observation per landmark
@@ -565,6 +571,7 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
         memcpy(vi, p.vis_frame_i, sizeof(int) * p.num_vis); memcpy(vj, p.vis_frame_j, sizeof(int) * p.num_vis);
         int run = -1;
         for (int i = 0; i < p.num_vis; i++) {
+            if (lo.dev_obs) { if (i == 0 || vl[i] != vl[i - 1]) run++; voi[i] = lo.obsi_off + run; continue; }      // one host side per landmark, filled on the device
             const double *o = p.vis_obs + (size_t)i * 12;
             double hi[6];
             split_obs(o, hi, oj + (size_t)i * 6);
@@ -669,7 +676,8 @@ static void lower_fill(const viwb_problem &p, const double *state, int w, const 
         memcpy(h.prior_J + pd.J_off, pr.J, sizeof(double) * pr.n * pr.n); memcpy(h.prior_r + pd.r_off, pr.r, sizeof(double) * pr.n);
         memcpy(h.prior_x0 + pd.x0_off, pr.x0, sizeof(double) * SFIX);
     }
-    memcpy(h.x_init + m.state_off, state, sizeof(double) * (SFIX + p.num_landmarks));
+    if (lo.dev_obs) { memcpy(h.x_fix + (size_t)SFIX * w, state, sizeof(double) * SFIX); h.fm_off[w] = m.state_off; h.fm_off[h.meta_count + w] = m.lm_off; }
+    else memcpy(h.x_init + m.state_off, state, sizeof(double) * (SFIX + p.num_landmarks));
     WinWork &ww = h.work[w]; memset(&ww, 0, sizeof ww);
     ww.status = ST_RUNNING; ww.phase = PH_INIT; ww.first = 1; ww.radius = init_radius; ww.mu = 1e-8; ww.mu_lin = 1e-8; ww.term = VIWB_NO_CONVERGENCE;
 }
@@ -686,13 +694,19 @@ template <typename F> static void parallel_for(int n, F f) {
     for (auto &t : th) t.join();
 }
 
+static void fm_fill_batch(viwb_features *fs, const viwb_batch *b);
+// from: the windows' visual tables are index tables rebuilt from these lists (viwb_features_batch_create), their observations and landmark states are
+// filled from the lists on the device after the upload, which leaves them out
 static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, const double *const *states,
-                       const viwb_options *options, const int32_t *margin_flags, viwb_batch **out, bool use_cached = false, bool obs_per_factor = false) {
+                       const viwb_options *options, const int32_t *margin_flags, viwb_batch **out, bool use_cached = false, bool obs_per_factor = false,
+                       viwb_features *from = nullptr) {
     bind_device(ctx);
     if (B <= 0 || !problems || !states) return fail(ctx, VIWB_ERR_INVALID, "empty batch");
     const double t_start = now_ms();
     viwb_batch *b = new viwb_batch();
     b->B = B; b->any_marg = false; b->algorithmic_bytes = 0; b->arena_cached = false; b->out_bytes = 0; b->prior_nmax = 0; b->work_init_dev = nullptr;
+    b->fs = nullptr; b->fs_gen = 0; b->x_fix = nullptr; b->fm_off = nullptr;
+    const bool dev_obs = from != nullptr;
     viwb_options defopt; viwb_default_options(&defopt);
     const viwb_options *opt = options ? options : &defopt;
     b->max_iter = opt->max_num_iterations;
@@ -703,7 +717,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     std::vector<WinLow> low(B);
     // ---- phase 1 (parallel): sizes and plans
     const bool allow_fused = getenv("VIWB_NO_FUSED") == nullptr;      // read once per build: every window of the batch is planned under the same switch
-    parallel_for(B, [&](int w) { lower_count(problems[w], margin_flags ? margin_flags[w] : -1, allow_fused, b->meta[w], low[w], b->out_mode[w]); });
+    parallel_for(B, [&](int w) { lower_count(problems[w], margin_flags ? margin_flags[w] : -1, allow_fused, dev_obs, b->meta[w], low[w], b->out_mode[w]); });
     const double t_counted = now_ms();
     if (obs_per_factor) for (int w = 0; w < B; w++) { low[w].obs_per_factor = true; low[w].nobs_i = problems[w].num_vis < 0 ? 0 : problems[w].num_vis; }
     for (int w = 0; w < B; w++) if (low[w].err) { const int e = low[w].err; batch_free(ctx, b); return fail(ctx, VIWB_ERR_INVALID, e == 1 ? "bad frame_count / num_landmarks" : e == 2 ? "bad prior" : e == 3 ? "bad visual factor table" : e == 5 ? "negative factor count or missing table" : "bad factor frame index"); }
@@ -795,17 +809,20 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     };
     auto WK = [&](auto **dev, size_t count) { ents.push_back({(void **)dev, nullptr, (count ? count : 1) * sizeof(**dev), 0}); };
     IN(&bd.meta, h.meta, B); IN(&bd.prior, h.prior, npri); IN(&bd.vis_code, h.vis_code, nvis); IN(&bd.vis_lm, h.vis_lm, nvis); IN(&bd.vis_oi, h.vis_oi, nvis);
-    IN(&bd.obs_i, h.obs_i, nobsi * 6); IN(&bd.obs_j, h.obs_j, nvis * 6); IN(&bd.lm_win, h.lm_win, nlm); IN(&bd.lm_fptr, h.lm_fptr, nlm + 1);
+    if (!dev_obs) { IN(&bd.obs_i, h.obs_i, nobsi * 6); IN(&bd.obs_j, h.obs_j, nvis * 6); }
+    IN(&bd.lm_win, h.lm_win, nlm); IN(&bd.lm_fptr, h.lm_fptr, nlm + 1);
     IN(&bd.items, h.items, nit_s + nit_m); IN(&bd.asm_list, h.asm_list, nlist);
     IN(&bd.imu_fi, h.imu_fi, nimu); IN(&bd.imu_fj, h.imu_fj, nimu); IN(&bd.imu_win, h.imu_win, nimu); IN(&bd.wheel_fi, h.wheel_fi, nwheel); IN(&bd.wheel_fj, h.wheel_fj, nwheel); IN(&bd.wheel_win, h.wheel_win, nwheel);
     IN(&bd.plane_f, h.plane_f, nplane); IN(&bd.plane_win, h.plane_win, nplane); IN(&bd.imu_data, h.imu_data, nimu * 287); IN(&bd.wheel_data, h.wheel_data, nwheel * 78);
-    IN(&bd.prior_J, h.prior_J, npJ); IN(&bd.prior_r, h.prior_r, npr); IN(&bd.prior_x0, h.prior_x0, npri * SFIX); IN(&bd.x_init, h.x_init, nstate); IN(&b->work_init_dev, h.work, B);
+    IN(&bd.prior_J, h.prior_J, npJ); IN(&bd.prior_r, h.prior_r, npr); IN(&bd.prior_x0, h.prior_x0, npri * SFIX); IN(&b->work_init_dev, h.work, B);
+    if (dev_obs) { IN(&b->x_fix, h.x_fix, (size_t)B * SFIX); IN(&b->fm_off, h.fm_off, 2 * (size_t)B); } else IN(&bd.x_init, h.x_init, nstate);
     IN(&bd.vis_pos, h.vis_pos, bd.n_fused_wide ? nvis : 0); IN(&bd.lmb_desc, h.lmb_desc, nlmb); IN(&bd.pitems, h.pitems, npit);
     IN(&bd.mvis_pos, h.mvis_pos, nmpit ? nvis : 0); IN(&bd.mpitems, h.mpitems, nmpit);
     int *h_plan = nullptr; IN(&bd.chol_plan, h_plan, nplan);
     IN(&bd.run_desc, h.run_desc, nrun); IN(&bd.run_tile, h.run_tile, nrtile); IN(&bd.run_f, h.run_f, nrun ? nvis : 0); IN(&bd.run_lm, h.run_lm, nrun ? 2 * nlm : 0);
     const size_t nvec = (size_t)B * TFIX + nlm;
     const bool any_unfused = bd.n_unfused || bd.n_munfused;      // lin_vis' per-factor records and costs
+    if (dev_obs) { WK(&bd.obs_i, nobsi * 6); WK(&bd.obs_j, nvis * 6); WK(&bd.x_init, nstate); }
     WK(&bd.work, B); WK(&bd.x_cur, nstate); WK(&bd.x_cand, nstate); WK(&bd.x_before, nstate);
     WK(&bd.vis_type, nvis); WK(&bd.vis_fi, nvis); WK(&bd.vis_fj, nvis); WK(&bd.vis_win, nvis); WK(&bd.vis_dup, nvis); WK(&bd.vis_obs, nvis * 12);
     WK(&bd.vis_rec, any_unfused ? nvis * VREC : 0); WK(&bd.vis_cost, any_unfused ? nvis : 0);
@@ -835,7 +852,7 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     if (b->arena_cached) b->arena = *ar;     // a view; ownership stays with the context
     const double t_alloc = now_ms();
     for (auto &e : ents) { *e.dev = ar->dev + e.off; if (e.host) *e.host = ar->host + e.off; }
-    h.nitems_solve_total = (int)nit_s;
+    h.nitems_solve_total = (int)nit_s; h.meta_count = B;
     if (npri) memcpy(h.prior, priors.data(), sizeof(PriorDev) * npri);
     h.lm_fptr[nlm] = (int)nvis;
     for (const std::vector<int> &pl : plans) { memcpy(h_plan, pl.data(), sizeof(int) * pl.size()); h_plan += pl.size(); }
@@ -844,11 +861,12 @@ static int batch_build(viwb_context *ctx, int B, const viwb_problem *problems, c
     parallel_for(B, [&](int w) { lower_fill(problems[w], states[w], w, b->meta[w], low[w], h, opt->initial_trust_region_radius); });
     if (!obs_per_factor && std::find(obs_viol.begin(), obs_viol.end(), 1) != obs_viol.end()) {      // rare: rebuild with one host-side entry per factor
         batch_free(ctx, b);
-        return batch_build(ctx, B, problems, states, options, margin_flags, out, use_cached, true);
+        return batch_build(ctx, B, problems, states, options, margin_flags, out, use_cached, true, from);
     }
     const double t_filled = now_ms();
     { int e = dev_h2d(ar->dev, ar->host, in_bytes, ctx->stream); if (e) { batch_free(ctx, b); return fail(ctx, VIWB_ERR_CUDA, std::string("H2D: ") + dev_errstr(e)); } }
     ctx->h2d_bytes += (long long)in_bytes;
+    if (dev_obs) fm_fill_batch(from, b);
     if (nvis) LAUNCH(ctx, vis_expand, bd, B, 1, NT(128), 0, 0);      // code words + split observations -> the tables the kernels read
     { const int rc = launch_status(ctx); if (rc) { batch_free(ctx, b); return rc; } }
     // (no wait here: the kernels of the run are queued behind the upload on the same stream, the results are staged in their own region of the slab, and the
@@ -1021,6 +1039,16 @@ static void batch_free(viwb_context *ctx, viwb_batch *b) {
     delete b;
 }
 
+// outliersRejection on the states the batch currently holds (after viwb_batch_run: the solved, re-anchored windows) -> bd.lm_outlier
+static int batch_outlier_launch(viwb_context *ctx, viwb_batch *b, double focal_length, double threshold_px) {
+    BatchDev bd = b->bd; bd.out_focal = focal_length; bd.out_thresh = threshold_px;
+    const int nt = NT(128);
+    LAUNCH(ctx, outlier, bd, (bd.nlm_total + nt - 1) / nt, 1, nt, 0, 0);
+    return launch_status(ctx);
+}
+
+#include "features_batch.inl"
+
 // ====================================================================================== C ABI
 extern "C" int viwb_create(int device, viwb_context **out) {
     if (!out) return VIWB_ERR_INVALID;
@@ -1137,14 +1165,12 @@ extern "C" int viwb_batch_download(viwb_context *ctx, viwb_batch *b, double *con
     if (!ctx || !b) return VIWB_ERR_INVALID;
     return batch_fetch(ctx, b, states, summaries, priors_out);
 }
-// outliersRejection on the states the batch currently holds (after viwb_batch_run: the solved, re-anchored windows)
+// outliersRejection on the states the batch currently holds, verdicts to the host
 extern "C" int viwb_batch_outliers(viwb_context *ctx, viwb_batch *b, double focal_length, double threshold_px, uint8_t *const *outliers) {
     if (!ctx || !b || !outliers) return VIWB_ERR_INVALID;
     bind_device(ctx);
-    BatchDev bd = b->bd; bd.out_focal = focal_length; bd.out_thresh = threshold_px;
-    const int nt = NT(128);
-    LAUNCH(ctx, outlier, bd, (bd.nlm_total + nt - 1) / nt, 1, nt, 0, 0);
-    const int rc = launch_status(ctx); if (rc) return rc;
+    const BatchDev &bd = b->bd;
+    const int rc = batch_outlier_launch(ctx, b, focal_length, threshold_px); if (rc) return rc;
     std::vector<int> h(bd.nlm_total > 0 ? bd.nlm_total : 1);
     CK(dev_d2h(h.data(), bd.lm_outlier, (size_t)bd.nlm_total * sizeof(int), ctx->stream));
     CK(dev_sync(ctx->stream));
@@ -1636,6 +1662,19 @@ extern "C" int viwb_features_remove_outliers(viwb_features *fs, const uint8_t *o
 extern "C" int viwb_features_predict(viwb_features *fs, const double *states, const int32_t *frame_count, int32_t *n_pred, int32_t *pred_ids, double *pred_pts_cam,
                                      uint8_t *has_prediction) {
     return fs ? fm_predict_run(fs, states, frame_count, n_pred, pred_ids, pred_pts_cam, has_prediction) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_batch_create(viwb_features *fs, const viwb_problem *problems, const double *states, const viwb_options *options,
+                                          const int32_t *margin_flags, int32_t *num_landmarks, viwb_batch **out) {
+    return fs ? fm_batch_create(fs, problems, states, options, margin_flags, num_landmarks, out) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_set_depth_batch(viwb_features *fs, const viwb_batch *b) { return fs ? fm_set_depth_batch(fs, b) : VIWB_ERR_INVALID; }
+extern "C" int viwb_features_remove_outliers_batch(viwb_features *fs, viwb_batch *b, double focal_length, double threshold_px, int32_t *n_removed,
+                                                   int32_t *removed_ids) {
+    return fs ? fm_remove_outliers_batch(fs, b, focal_length, threshold_px, n_removed, removed_ids) : VIWB_ERR_INVALID;
+}
+extern "C" int viwb_features_predict_batch(viwb_features *fs, const viwb_batch *b, const int32_t *frame_count, int32_t *n_pred, int32_t *pred_ids,
+                                           double *pred_pts_cam, uint8_t *has_prediction) {
+    return fs ? fm_predict_batch(fs, b, frame_count, n_pred, pred_ids, pred_pts_cam, has_prediction) : VIWB_ERR_INVALID;
 }
 extern "C" int viwb_features_slide(viwb_features *fs, const int32_t *frame_count, const uint8_t *shift_depth, const double *marg_R, const double *marg_P,
                                    const double *new_R, const double *new_P) {

@@ -26,7 +26,8 @@ EXPORTS = ["viwb_create", "viwb_destroy", "viwb_last_error", "viwb_set_stream", 
            "viwb_solve_gyroscope_bias", "viwb_linear_alignment",
            "viwb_features_create", "viwb_features_destroy", "viwb_features_add", "viwb_features_add_tracked", "viwb_features_decisions", "viwb_features_triangulate",
            "viwb_features_window", "viwb_features_set_depth", "viwb_features_remove_outliers", "viwb_features_predict", "viwb_features_slide",
-           "viwb_features_remove_failures", "viwb_features_download"]
+           "viwb_features_remove_failures", "viwb_features_download", "viwb_features_batch_create", "viwb_features_set_depth_batch",
+           "viwb_features_remove_outliers_batch", "viwb_features_predict_batch"]
 
 
 class ViwbError(RuntimeError):
@@ -622,11 +623,39 @@ class Features:
         n, ids, pts, hp = np.zeros(self.F, np.int32), np.zeros(self.F * self.M, np.int32), np.zeros((self.F * self.M, 3)), np.zeros(self.F, np.uint8)
         vp = self._vp
         self._call("viwb_features_predict", vp(st), vp(fc), vp(n), vp(ids), vp(pts), vp(hp))
+        return self._predictions(n, ids, pts, hp)
+
+    def _predictions(self, n, ids, pts, hp):
         out, o = [], 0
         for s in range(self.F):
             out.append((ids[o: o + n[s]].copy(), pts[o: o + n[s]].copy()) if hp[s] else None)
             o += n[s]
         return out
+
+    def batch(self, problems, states, flags=None, options=None):
+        """viwb_features_batch_create: one window per stream, its visual table and landmark inverse depths taken from the lists on the device.
+        problems[s]: abi.WindowProblem with everything but the visual table (num_landmarks 0); states [streams, 207] -> a Batch whose download /
+        outliers size each window by the landmark count the lists gave it (Batch.num_landmarks)."""
+        assert len(problems) == self.F
+        return Batch(self.ctx, problems, states, flags, options, features=self)
+
+    def set_depth_from(self, batch):
+        """setDepth from the batch's current landmark states (viwb_features_set_depth_batch)"""
+        self._call("viwb_features_set_depth_batch", batch.h)
+
+    def remove_outliers_from(self, batch, focal=460.0, thresh=3.0):
+        """outliersRejection on the batch + removeOutlier (viwb_features_remove_outliers_batch) -> per stream the removed ids, ascending"""
+        n, ids = np.zeros(self.F, np.int32), np.zeros((self.F, self.M), np.int32)
+        self._call("viwb_features_remove_outliers_batch", batch.h, C.c_double(focal), C.c_double(thresh), self._vp(n), self._vp(ids))
+        return [ids[s, : n[s]].copy() for s in range(self.F)]
+
+    def predict_from(self, batch, frame_count):
+        """predict() with each stream's fixed state read from the batch (viwb_features_predict_batch)"""
+        fc = self._per_stream(frame_count, np.int32)
+        n, ids, pts, hp = np.zeros(self.F, np.int32), np.zeros(self.F * self.M, np.int32), np.zeros((self.F * self.M, 3)), np.zeros(self.F, np.uint8)
+        vp = self._vp
+        self._call("viwb_features_predict_batch", batch.h, vp(fc), vp(n), vp(ids), vp(pts), vp(hp))
+        return self._predictions(n, ids, pts, hp)
 
     def slide(self, frame_count, shift_depth, marg_R=None, marg_P=None, new_R=None, new_P=None):
         fc, sh = self._per_stream(frame_count, np.int32), self._per_stream(shift_depth, np.uint8)
@@ -776,21 +805,34 @@ class LkBatch:
 
 
 class Batch:
-    """Device-resident batch of windows: upload once, run many times."""
+    """Device-resident batch of windows: upload once, run many times.  features: a Features whose lists supply the visual tables
+    (viwb_features_batch_create; Features.batch), else viwb_batch_create with the problems' own."""
 
-    def __init__(self, ctx, problems, states, flags=None, options=None):
+    def __init__(self, ctx, problems, states, flags=None, options=None, features=None):
         self.ctx = ctx
         self.B = len(problems)
         self.problems = problems
         self._arr = (abi.Problem * self.B)()
         for i, p in enumerate(problems):
             p.fill(self._arr[i])
-        self._states = [np.ascontiguousarray(s, np.float64) for s in states]
-        sp = (abi.c_double_p * self.B)(*[_dp(s) for s in self._states])
         fl = (C.c_int32 * self.B)(*[int(f) for f in flags]) if flags is not None else None
         opt = options if options is not None else abi.default_options()
         self.h = C.c_void_p()
-        ctx._ck(ctx.lib.viwb_batch_create(ctx.h, C.c_int(self.B), self._arr, sp, C.byref(opt), fl, C.byref(self.h)), "viwb_batch_create")
+        if features is None:
+            self._states = [np.ascontiguousarray(s, np.float64) for s in states]
+            sp = (abi.c_double_p * self.B)(*[_dp(s) for s in self._states])
+            self.num_landmarks = [p.num_landmarks for p in problems]
+            ctx._ck(ctx.lib.viwb_batch_create(ctx.h, C.c_int(self.B), self._arr, sp, C.byref(opt), fl, C.byref(self.h)), "viwb_batch_create")
+            return
+        for i, p in enumerate(problems):          # the lists supply the visual tables: an empty one is passed as NULL
+            if len(p.vis_type) == 0:
+                a = self._arr[i]
+                a.vis_type = a.vis_landmark = a.vis_frame_i = a.vis_frame_j = None
+                a.vis_obs = None
+        self._states = np.ascontiguousarray(np.asarray(states, np.float64).reshape(self.B, abi.STATE_FIXED))
+        nlm = np.zeros(self.B, np.int32)
+        features._call("viwb_features_batch_create", self._arr, _dp(self._states), C.byref(opt), fl, nlm.ctypes.data_as(C.c_void_p), C.byref(self.h))
+        self.num_landmarks = [int(x) for x in nlm]
 
     def run(self):
         self.ctx._ck(self.ctx.lib.viwb_batch_run(self.ctx.h, self.h), "viwb_batch_run")
@@ -810,7 +852,7 @@ class Batch:
         return nt.value, sm.value, (bps.value if occupancy else None)
 
     def download(self, want_priors=True):
-        sts = [np.zeros(p.state_size) for p in self.problems]
+        sts = [np.zeros(abi.STATE_FIXED + n) for n in self.num_landmarks]
         sp = (abi.c_double_p * self.B)(*[_dp(s) for s in sts])
         summ = (abi.Summary * self.B)()
         pri = [abi.PriorData() for _ in range(self.B)] if want_priors else None
@@ -829,10 +871,10 @@ class Batch:
 
     def outliers(self, focal=460.0, thresh=3.0):
         """Estimator::outliersRejection on the windows as the batch currently holds them (call after run())."""
-        outs = [np.zeros(max(p.num_landmarks, 1), np.uint8) for p in self.problems]
+        outs = [np.zeros(max(n, 1), np.uint8) for n in self.num_landmarks]
         arr = (C.c_void_p * self.B)(*[o.ctypes.data for o in outs])
         self.ctx._ck(self.ctx.lib.viwb_batch_outliers(self.ctx.h, self.h, C.c_double(focal), C.c_double(thresh), arr), "viwb_batch_outliers")
-        return [o[: p.num_landmarks] for o, p in zip(outs, self.problems)]
+        return [o[:n] for o, n in zip(outs, self.num_landmarks)]
 
     def destroy(self):
         if self.h:
